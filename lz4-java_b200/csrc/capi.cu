@@ -21,8 +21,7 @@
 
 namespace b200 {
 
-static std::atomic<unsigned long long> g_launches{0};
-std::atomic<unsigned long long> g_launch_count{0};      // launches made by frame.cu / containers.cu
+std::atomic<unsigned long long> g_launch_count{0};
 static thread_local char tl_err[256] = "";
 static thread_local int tl_status = 0;          // B200LZ4_E_* of the last value-returning call (hashes, digests) on this thread
 static thread_local int tl_device = -1;          // -1: not chosen yet (defaults to device 0)
@@ -56,7 +55,23 @@ static int ensure_device()
 }
 
 // ---------------------------------------------------------------------------------------------
-// A pipeline slot: one stream, device staging for a chunk of blocks and pinned descriptor arrays.
+// Per-block descriptors of one chunk: [total | soff | doff | out] u64, [slen | dcap | res] i32, for nb blocks.
+// `out` is what the device hands back per block besides `res`: the packed offsets (compact) or the hashes.
+struct Desc {
+    uint8_t* base = nullptr; size_t cap = 0;           // allocation, in bytes
+    size_t nb = 0;                                     // blocks the layout is cut for
+    uint64_t* total() const { return (uint64_t*)base; }
+    uint64_t* soff() const { return (uint64_t*)base + 2; }
+    uint64_t* doff() const { return soff() + nb; }
+    uint64_t* out()  const { return soff() + 2 * nb; }
+    int32_t*  slen() const { return (int32_t*)(soff() + 3 * nb); }
+    int32_t*  dcap() const { return slen() + nb; }
+    int32_t*  res()  const { return slen() + 2 * nb; }
+    static size_t bytes(size_t nb) { return 16 + nb * (3 * 8 + 3 * 4); }
+    size_t bytes() const { return bytes(nb); }
+};
+
+// A pipeline slot: one stream, device staging for a chunk of blocks and its descriptors, pinned and on the device.
 struct Slot {
     cudaStream_t st = nullptr;
     cudaEvent_t done = nullptr;
@@ -65,25 +80,9 @@ struct Slot {
     uint8_t* h_out = nullptr; size_t h_out_cap = 0;    // pinned bounce for scattered dst slots
     bool scatter = false;                              // retire must copy h_out -> caller slots
     cudaEvent_t drained = nullptr; bool draining = false;
-    // descriptors: [total | soff | doff | xoff] u64, [slen | dcap | res] i32 — one pinned and one device copy
-    uint8_t *h_desc = nullptr, *d_desc = nullptr; size_t desc_blocks = 0;
+    Desc h, d;                                         // same layout: h is pinned, d its device copy
     size_t i0 = 0, i1 = 0;            // block range in flight
     bool busy = false;
-    uint64_t* h_total() const { return (uint64_t*)h_desc; }
-    uint64_t* h_soff() const { return (uint64_t*)h_desc + 2; }
-    uint64_t* h_doff() const { return h_soff() + desc_blocks; }
-    uint64_t* h_xoff() const { return h_soff() + 2 * desc_blocks; }
-    int32_t*  h_slen() const { return (int32_t*)(h_soff() + 3 * desc_blocks); }
-    int32_t*  h_dcap() const { return h_slen() + desc_blocks; }
-    int32_t*  h_res()  const { return h_slen() + 2 * desc_blocks; }
-    uint64_t* d_total() const { return (uint64_t*)d_desc; }
-    uint64_t* d_soff() const { return (uint64_t*)d_desc + 2; }
-    uint64_t* d_doff() const { return d_soff() + desc_blocks; }
-    uint64_t* d_xoff() const { return d_soff() + 2 * desc_blocks; }
-    int32_t*  d_slen() const { return (int32_t*)(d_soff() + 3 * desc_blocks); }
-    int32_t*  d_dcap() const { return d_slen() + desc_blocks; }
-    int32_t*  d_res()  const { return d_slen() + 2 * desc_blocks; }
-    static size_t desc_bytes(size_t nb) { return 16 + nb * (3 * 8 + 3 * 4); }
 };
 
 static constexpr int    NSLOTS = 3;
@@ -178,45 +177,48 @@ struct PipelineGuard {
     ~PipelineGuard() { if (!completed) ctx_abandon(c); }
 };
 
+// Grow-or-keep staging: a buffer smaller than `need` bytes is replaced by one with need >> slack_shift more room plus
+// 4 KiB, so calls of about the same size keep their buffers.  Whatever still reads or writes the old buffer must be done.
+static int reserve_device(uint8_t*& p, size_t& cap, size_t need, int slack_shift = 2)
+{
+    if (need <= cap) return 0;
+    if (p) CK(cudaFree(p));
+    p = nullptr; cap = 0;
+    const size_t c = need + (need >> slack_shift) + 4096;
+    CK(cudaMalloc(&p, c)); cap = c;
+    return 0;
+}
+static int reserve_pinned(uint8_t*& p, size_t& cap, size_t need)
+{
+    if (need <= cap) return 0;
+    if (p) CK(cudaFreeHost(p));
+    p = nullptr; cap = 0;
+    const size_t c = need + (need >> 2) + 4096;
+    CK(cudaHostAlloc(&p, c, cudaHostAllocDefault)); cap = c;
+    return 0;
+}
+
 static int slot_reserve(Slot& s, size_t src_bytes, size_t dst_bytes, size_t nblocks, size_t aux_bytes = 0)
 {
     if (s.draining) { CK(cudaEventSynchronize(s.drained)); s.draining = false; }
-    if (aux_bytes > s.aux_cap) {
-        if (s.d_aux) CK(cudaFree(s.d_aux));
-        s.aux_cap = 0; s.d_aux = nullptr;
-        size_t cap = aux_bytes + (aux_bytes >> 2) + 4096;
-        CK(cudaMalloc(&s.d_aux, cap)); s.aux_cap = cap;
-    }
-    if (src_bytes > s.src_cap) {
-        if (s.d_src) CK(cudaFree(s.d_src));
-        s.src_cap = 0; s.d_src = nullptr;
-        size_t cap = src_bytes + (src_bytes >> 2) + 4096;
-        CK(cudaMalloc(&s.d_src, cap)); s.src_cap = cap;
-    }
-    if (dst_bytes > s.dst_cap) {
-        if (s.d_dst) CK(cudaFree(s.d_dst));
-        s.dst_cap = 0; s.d_dst = nullptr;
-        size_t cap = dst_bytes + (dst_bytes >> 2) + 4096;
-        CK(cudaMalloc(&s.d_dst, cap)); s.dst_cap = cap;
-    }
-    if (nblocks > s.desc_blocks) {
-        if (s.d_desc) CK(cudaFree(s.d_desc));
-        if (s.h_desc) CK(cudaFreeHost(s.h_desc));
-        s.d_desc = nullptr; s.h_desc = nullptr; s.desc_blocks = 0;
-        size_t nb = nblocks + (nblocks >> 1) + 64;
-        nb = (nb + 1) & ~size_t(1);                    // keeps the i32 arrays 8-byte aligned
-        CK(cudaMalloc(&s.d_desc, Slot::desc_bytes(nb)));
-        CK(cudaHostAlloc(&s.h_desc, Slot::desc_bytes(nb), cudaHostAllocDefault));
-        s.desc_blocks = nb;
-    }
-    return 0;
+    int rc = reserve_device(s.d_aux, s.aux_cap, aux_bytes);
+    if (!rc) rc = reserve_device(s.d_src, s.src_cap, src_bytes);
+    if (!rc) rc = reserve_device(s.d_dst, s.dst_cap, dst_bytes);
+    if (rc || nblocks <= s.h.nb) return rc;
+    size_t nb = nblocks + (nblocks >> 1) + 64;
+    nb = (nb + 1) & ~size_t(1);                        // keeps the i32 arrays 8-byte aligned
+    s.h.nb = s.d.nb = 0;                               // a failed reserve below frees the old buffer: the next call must allocate
+    rc = reserve_device(s.d.base, s.d.cap, Desc::bytes(nb));
+    if (!rc) rc = reserve_pinned(s.h.base, s.h.cap, Desc::bytes(nb));
+    if (!rc) s.h.nb = s.d.nb = nb;
+    return rc;
 }
 
 enum Op { OP_COMPRESS_FAST, OP_COMPRESS_HC, OP_DEC_SAFE, OP_DEC_FAST };
 
 static cudaError_t launch_op(Op op, const BatchArgs& a, int param, cudaStream_t st)
 {
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     switch (op) {
     case OP_COMPRESS_FAST: return launch_compress_fast(a, param, st);
     case OP_COMPRESS_HC:   return launch_compress_hc(a, param, st);
@@ -225,21 +227,56 @@ static cudaError_t launch_op(Op op, const BatchArgs& a, int param, cudaStream_t 
     }
 }
 
-// finish the slot's in-flight chunk: wait, hand the per-block results (and, for scattered dst
-// layouts, the bytes staged in the pinned bounce buffer) to the caller
-static int slot_retire(Slot& s, int32_t* result, uint8_t* dst_base = nullptr, const uint64_t* dst_off = nullptr,
-                       const int32_t* dst_cap = nullptr)
+// One chunk of a host-buffer call: blocks [i0, i0 + nb), their source bytes [s_lo, s_lo + s_span) and, when the call
+// has dst slots, their dst bytes [d_lo, d_lo + d_span).
+struct Chunk { size_t i0, nb; uint64_t s_lo, d_lo; size_t s_span, d_span; };
+
+// The host-buffer pipeline every host-buffer call runs.  It cuts blocks [0, n) into chunks of at most CHUNK_BLOCKS blocks
+// and CHUNK_SPAN bytes of source (and of dst, when dst_off is given) and runs them round-robin over the NSLOTS streams:
+//   stage(Slot&, const Chunk&)  reserves the slot's buffers and queues the chunk's copies in, its launches and its copies
+//                               back on s.st; the driver then records s.done;
+//   retire(Slot&)               hands the chunk [s.i0, s.i1) back to the caller, after s.done.
+// A slot's chunk is retired before the slot takes the next one and the last ones in block order, so results come back in
+// block order; the call returns after every `drained` event a retire recorded.  Blocks must ascend in src (and in dst,
+// without overlapping there); order_msg is the error otherwise.
+template <class Stage, class Retire>
+static int run_pipeline(size_t n, const uint64_t* src_off, const int32_t* src_len, const uint64_t* dst_off,
+                        const int32_t* dst_cap, const char* order_msg, Stage stage, Retire retire)
 {
-    if (!s.busy) return 0;
-    CK(cudaEventSynchronize(s.done));
-    memcpy(result + s.i0, s.h_res(), (s.i1 - s.i0) * sizeof(int32_t));
-    if (s.scatter && dst_base) {
-        const uint64_t d_lo = dst_off[s.i0];
-        for (size_t k = s.i0; k < s.i1; k++)
-            if (dst_cap[k] > 0) memcpy(dst_base + dst_off[k], s.h_out + (dst_off[k] - d_lo), (size_t)dst_cap[k]);
+    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
+    PipelineGuard guard(c);
+    auto finish = [&](Slot& s) -> int {
+        if (!s.busy) return 0;
+        CK(cudaEventSynchronize(s.done));
+        const int r = retire(s); if (r) return r;
+        s.busy = false;
+        return 0;
+    };
+    size_t i0 = 0; int cur = 0;
+    while (i0 < n) {
+        // ---- pick the chunk [i0, i1).  Negative sizes span no bytes: they are per-block errors in the reference
+        // (lz4.c:1324, 1953), and the kernels report them.
+        const uint64_t s_lo = src_off[i0], d_lo = dst_off ? dst_off[i0] : 0;
+        uint64_t s_hi = s_lo, d_hi = d_lo;
+        size_t i1 = i0;
+        while (i1 < n && i1 - i0 < CHUNK_BLOCKS) {
+            if (src_off[i1] < s_lo || (dst_off && (dst_off[i1] < d_lo || (i1 > i0 && dst_off[i1] < d_hi)))) return fail_arg(order_msg);
+            const uint64_t se = src_off[i1] + (uint64_t)(src_len[i1] > 0 ? src_len[i1] : 0);
+            const uint64_t de = dst_off ? dst_off[i1] + (uint64_t)(dst_cap[i1] > 0 ? dst_cap[i1] : 0) : 0;
+            const uint64_t ns = se > s_hi ? se : s_hi, nd = de > d_hi ? de : d_hi;
+            if (i1 > i0 && (ns - s_lo > CHUNK_SPAN || nd - d_lo > CHUNK_SPAN)) break;
+            s_hi = ns; d_hi = nd; i1++;
+        }
+        Slot& s = c->slot[cur];
+        rc = finish(s); if (rc) return rc;
+        rc = stage(s, Chunk{ i0, i1 - i0, s_lo, d_lo, (size_t)(s_hi - s_lo), (size_t)(d_hi - d_lo) }); if (rc) return rc;
+        CK(cudaEventRecord(s.done, s.st));
+        s.busy = true; s.i0 = i0; s.i1 = i1;
+        i0 = i1; cur = (cur + 1) % NSLOTS;
     }
-    s.scatter = false;
-    s.busy = false;
+    for (int k = 0; k < NSLOTS; k++) { rc = finish(c->slot[(cur + k) % NSLOTS]); if (rc) return rc; }
+    for (Slot& s : c->slot) if (s.draining) { CK(cudaEventSynchronize(s.drained)); s.draining = false; }
+    guard.completed = true;
     return 0;
 }
 
@@ -250,86 +287,61 @@ static int host_batch(Op op, const uint8_t* src_base, const uint64_t* src_off, c
 {
     if (n == 0) return 0;
     if (!src_base || !src_off || !src_len || !dst_base || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
-    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
-    PipelineGuard guard(c);
-
-    size_t i0 = 0; int cur = 0;
-    while (i0 < n) {
-        // ---- pick the chunk [i0, i1): bounded block count and bounded src/dst spans
-        const uint64_t s_lo = src_off[i0], d_lo = dst_off[i0];
-        uint64_t s_hi = s_lo, d_hi = d_lo;
-        size_t i1 = i0;
-        while (i1 < n && i1 - i0 < CHUNK_BLOCKS) {
-            if (src_len[i1] < 0 || dst_cap[i1] < 0) {
-                // negative sizes are per-block errors in the reference (lz4.c:1324, 1953); let the kernel report them
-            }
-            const uint64_t se = src_off[i1] + (uint64_t)(src_len[i1] > 0 ? src_len[i1] : 0);
-            const uint64_t de = dst_off[i1] + (uint64_t)(dst_cap[i1] > 0 ? dst_cap[i1] : 0);
-            if (src_off[i1] < s_lo || dst_off[i1] < d_lo || (i1 > i0 && dst_off[i1] < d_hi))
-                return fail_arg("blocks must ascend and not overlap in dst");
-            const uint64_t ns = se > s_hi ? se : s_hi, nd = de > d_hi ? de : d_hi;
-            if (i1 > i0 && (ns - s_lo > CHUNK_SPAN || nd - d_lo > CHUNK_SPAN)) break;
-            s_hi = ns; d_hi = nd; i1++;
-        }
-        const size_t nb = i1 - i0, s_span = (size_t)(s_hi - s_lo), d_span = (size_t)(d_hi - d_lo);
-
-        Slot& s = c->slot[cur];
-        rc = slot_retire(s, result, dst_base, dst_off, dst_cap); if (rc) return rc;
-        rc = slot_reserve(s, s_span + 16, d_span + 16, nb); if (rc) return rc;
-
+    auto stage = [&](Slot& s, const Chunk& ch) -> int {
+        int rc = slot_reserve(s, ch.s_span + 16, ch.d_span + 16, ch.nb); if (rc) return rc;
         // keep the source's 16-byte phase so aligned inputs stay aligned on the device
-        const size_t s_phase = (size_t)((uintptr_t)(src_base + s_lo) & 15), d_phase = (size_t)((uintptr_t)(dst_base + d_lo) & 15);
-        for (size_t k = 0; k < nb; k++) {
-            s.h_soff()[k] = src_off[i0 + k] - s_lo + s_phase;
-            s.h_doff()[k] = dst_off[i0 + k] - d_lo + d_phase;
-            s.h_slen()[k] = src_len[i0 + k];
-            s.h_dcap()[k] = dst_cap[i0 + k];
+        const size_t s_phase = (size_t)((uintptr_t)(src_base + ch.s_lo) & 15), d_phase = (size_t)((uintptr_t)(dst_base + ch.d_lo) & 15);
+        for (size_t k = 0; k < ch.nb; k++) {
+            s.h.soff()[k] = src_off[ch.i0 + k] - ch.s_lo + s_phase;
+            s.h.doff()[k] = dst_off[ch.i0 + k] - ch.d_lo + d_phase;
+            s.h.slen()[k] = src_len[ch.i0 + k];
+            s.h.dcap()[k] = dst_cap[ch.i0 + k];
         }
-        CK(cudaMemcpyAsync(s.d_desc, s.h_desc, Slot::desc_bytes(s.desc_blocks), cudaMemcpyHostToDevice, s.st));
-        if (s_span) CK(cudaMemcpyAsync(s.d_src + s_phase, src_base + s_lo, s_span, cudaMemcpyHostToDevice, s.st));
-        BatchArgs a{ s.d_src, s.d_soff(), s.d_slen(), s.d_dst, s.d_doff(), s.d_dcap(), s.d_res(), nb };
+        CK(cudaMemcpyAsync(s.d.base, s.h.base, s.h.bytes(), cudaMemcpyHostToDevice, s.st));
+        if (ch.s_span) CK(cudaMemcpyAsync(s.d_src + s_phase, src_base + ch.s_lo, ch.s_span, cudaMemcpyHostToDevice, s.st));
+        BatchArgs a{ s.d_src, s.d.soff(), s.d.slen(), s.d_dst, s.d.doff(), s.d.dcap(), s.d.res(), ch.nb };
         CK(launch_op(op, a, param, s.st));
-        CK(cudaMemcpyAsync(s.h_res(), s.d_res(), nb * sizeof(int32_t), cudaMemcpyDeviceToHost, s.st));
-        // copy back: when the dst slots are back to back (the normal layout) one DMA lands straight in
-        // the caller's memory; otherwise the span goes to a pinned bounce buffer and retire() scatters
-        // the slots, so caller bytes BETWEEN non-adjacent slots are never touched
-        bool contiguous = true;
-        {
-            uint64_t end = d_lo;
-            for (size_t k = 0; k < nb && contiguous; k++) {
-                if (dst_off[i0 + k] != end) contiguous = false;
-                end = dst_off[i0 + k] + (uint64_t)(dst_cap[i0 + k] > 0 ? dst_cap[i0 + k] : 0);
-            }
-        }
-        if (d_span && n == 1) {
+        CK(cudaMemcpyAsync(s.h.res(), s.d.res(), ch.nb * sizeof(int32_t), cudaMemcpyDeviceToHost, s.st));
+        if (!ch.d_span) return 0;
+        if (n == 1) {
             // one block per call (the JNI shim's shape): the caller's bytes behind the result stay untouched, like in the
             // reference (a decoder called with maxDestLen = "rest of my buffer" must not clobber what lies further along),
             // and no stale staging bytes of another call leave the device.  Costs one more round trip of a few bytes.
             CK(cudaStreamSynchronize(s.st));
-            const int32_t r = s.h_res()[0];
-            const size_t produced = op == OP_DEC_FAST ? (r >= 0 ? d_span : 0) : (size_t)(r > 0 ? r : 0);
-            if (produced) CK(cudaMemcpyAsync(dst_base + d_lo, s.d_dst + d_phase, produced < d_span ? produced : d_span, cudaMemcpyDeviceToHost, s.st));
-        } else if (d_span) {
-            if (contiguous) {
-                CK(cudaMemcpyAsync(dst_base + d_lo, s.d_dst + d_phase, d_span, cudaMemcpyDeviceToHost, s.st));
-            } else {
-                if (d_span > s.h_out_cap) {
-                    if (s.h_out) CK(cudaFreeHost(s.h_out));
-                    s.h_out = nullptr; s.h_out_cap = 0;
-                    const size_t cap = d_span + (d_span >> 2) + 4096;
-                    CK(cudaHostAlloc(&s.h_out, cap, cudaHostAllocDefault)); s.h_out_cap = cap;
-                }
-                CK(cudaMemcpyAsync(s.h_out, s.d_dst + d_phase, d_span, cudaMemcpyDeviceToHost, s.st));
-                s.scatter = true;
-            }
+            const int32_t r = s.h.res()[0];
+            const size_t produced = op == OP_DEC_FAST ? (r >= 0 ? ch.d_span : 0) : (size_t)(r > 0 ? r : 0);
+            if (produced) CK(cudaMemcpyAsync(dst_base + ch.d_lo, s.d_dst + d_phase, produced < ch.d_span ? produced : ch.d_span, cudaMemcpyDeviceToHost, s.st));
+            return 0;
         }
-        CK(cudaEventRecord(s.done, s.st));
-        s.busy = true; s.i0 = i0; s.i1 = i1;
-        i0 = i1; cur = (cur + 1) % NSLOTS;
-    }
-    for (int k = 0; k < NSLOTS; k++) { rc = slot_retire(c->slot[(cur + k) % NSLOTS], result, dst_base, dst_off, dst_cap); if (rc) return rc; }
-    guard.completed = true;
-    return 0;
+        // copy back: when the dst slots are back to back (the normal layout) one DMA lands straight in
+        // the caller's memory; otherwise the span goes to a pinned bounce buffer and retire scatters
+        // the slots, so caller bytes BETWEEN non-adjacent slots are never touched
+        bool contiguous = true;
+        uint64_t end = ch.d_lo;
+        for (size_t k = ch.i0; k < ch.i0 + ch.nb && contiguous; k++) {
+            if (dst_off[k] != end) contiguous = false;
+            end = dst_off[k] + (uint64_t)(dst_cap[k] > 0 ? dst_cap[k] : 0);
+        }
+        if (contiguous) {
+            CK(cudaMemcpyAsync(dst_base + ch.d_lo, s.d_dst + d_phase, ch.d_span, cudaMemcpyDeviceToHost, s.st));
+        } else {
+            rc = reserve_pinned(s.h_out, s.h_out_cap, ch.d_span); if (rc) return rc;
+            CK(cudaMemcpyAsync(s.h_out, s.d_dst + d_phase, ch.d_span, cudaMemcpyDeviceToHost, s.st));
+            s.scatter = true;
+        }
+        return 0;
+    };
+    auto retire = [&](Slot& s) -> int {
+        memcpy(result + s.i0, s.h.res(), (s.i1 - s.i0) * sizeof(int32_t));
+        if (s.scatter) {
+            const uint64_t d_lo = dst_off[s.i0];
+            for (size_t k = s.i0; k < s.i1; k++)
+                if (dst_cap[k] > 0) memcpy(dst_base + dst_off[k], s.h_out + (dst_off[k] - d_lo), (size_t)dst_cap[k]);
+            s.scatter = false;
+        }
+        return 0;
+    };
+    return run_pipeline(n, src_off, src_len, dst_off, dst_cap, "blocks must ascend and not overlap in dst", stage, retire);
 }
 
 template <typename W>
@@ -338,50 +350,23 @@ static int hash_host_batch(int bits, const uint8_t* base, const uint64_t* off, c
 {
     if (n == 0) return 0;
     if (!base || !off || !len || !out) return fail_arg("null pointer");
-    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
-    PipelineGuard guard(c);
-    size_t i0 = 0; int cur = 0;
-    while (i0 < n) {
-        const uint64_t lo = off[i0]; uint64_t hi = lo; size_t i1 = i0;
-        while (i1 < n && i1 - i0 < CHUNK_BLOCKS) {
-            if (off[i1] < lo) return fail_arg("buffers must ascend");
-            const uint64_t e = off[i1] + (uint64_t)(len[i1] > 0 ? len[i1] : 0);
-            const uint64_t nh = e > hi ? e : hi;
-            if (i1 > i0 && nh - lo > CHUNK_SPAN) break;
-            hi = nh; i1++;
-        }
-        const size_t nb = i1 - i0, span = (size_t)(hi - lo);
-        Slot& s = c->slot[cur];
-        if (s.busy) {
-            CK(cudaEventSynchronize(s.done));
-            memcpy(out + s.i0, s.h_doff(), (s.i1 - s.i0) * sizeof(W));   // h_doff doubles as the pinned result area
-            s.busy = false;
-        }
-        rc = slot_reserve(s, span + 16, 16, nb); if (rc) return rc;
-        const size_t phase = (size_t)((uintptr_t)(base + lo) & 15);
-        for (size_t k = 0; k < nb; k++) { s.h_soff()[k] = off[i0 + k] - lo + phase; s.h_slen()[k] = len[i0 + k]; }
-        CK(cudaMemcpyAsync(s.d_desc, s.h_desc, Slot::desc_bytes(s.desc_blocks), cudaMemcpyHostToDevice, s.st));
-        if (span) CK(cudaMemcpyAsync(s.d_src + phase, base + lo, span, cudaMemcpyHostToDevice, s.st));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        if (bits == 32) CK((span / nb >= 32768 ? launch_xxh32_long : launch_xxh32)(            // few long streams: one warp each
-                               s.d_src, s.d_soff(), s.d_slen(), (uint32_t)seed, (uint32_t*)s.d_doff(), nb, s.st));
-        else            CK((span / nb >= 32768 ? launch_xxh64_long : launch_xxh64)(
-                               s.d_src, s.d_soff(), s.d_slen(), seed, (uint64_t*)s.d_doff(), nb, s.st));
-        CK(cudaMemcpyAsync(s.h_doff(), s.d_doff(), nb * sizeof(W), cudaMemcpyDeviceToHost, s.st));
-        CK(cudaEventRecord(s.done, s.st));
-        s.busy = true; s.i0 = i0; s.i1 = i1;
-        i0 = i1; cur = (cur + 1) % NSLOTS;
-    }
-    for (int k = 0; k < NSLOTS; k++) {
-        Slot& s = c->slot[(cur + k) % NSLOTS];
-        if (s.busy) {
-            CK(cudaEventSynchronize(s.done));
-            memcpy(out + s.i0, s.h_doff(), (s.i1 - s.i0) * sizeof(W));
-            s.busy = false;
-        }
-    }
-    guard.completed = true;
-    return 0;
+    auto stage = [&](Slot& s, const Chunk& ch) -> int {
+        int rc = slot_reserve(s, ch.s_span + 16, 16, ch.nb); if (rc) return rc;
+        const size_t phase = (size_t)((uintptr_t)(base + ch.s_lo) & 15);
+        for (size_t k = 0; k < ch.nb; k++) { s.h.soff()[k] = off[ch.i0 + k] - ch.s_lo + phase; s.h.slen()[k] = len[ch.i0 + k]; }
+        CK(cudaMemcpyAsync(s.d.base, s.h.base, s.h.bytes(), cudaMemcpyHostToDevice, s.st));
+        if (ch.s_span) CK(cudaMemcpyAsync(s.d_src + phase, base + ch.s_lo, ch.s_span, cudaMemcpyHostToDevice, s.st));
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        const bool few_long = ch.s_span / ch.nb >= XXH_LONG_AVG;
+        if (bits == 32) CK((few_long ? launch_xxh32_long : launch_xxh32)(
+                               s.d_src, s.d.soff(), s.d.slen(), (uint32_t)seed, (uint32_t*)s.d.out(), ch.nb, s.st));
+        else            CK((few_long ? launch_xxh64_long : launch_xxh64)(
+                               s.d_src, s.d.soff(), s.d.slen(), seed, s.d.out(), ch.nb, s.st));
+        CK(cudaMemcpyAsync(s.h.out(), s.d.out(), ch.nb * sizeof(W), cudaMemcpyDeviceToHost, s.st));
+        return 0;
+    };
+    auto retire = [&](Slot& s) -> int { memcpy(out + s.i0, s.h.out(), (s.i1 - s.i0) * sizeof(W)); return 0; };
+    return run_pipeline(n, off, len, nullptr, nullptr, "buffers must ascend", stage, retire);
 }
 
 // one block, host buffers: the n = 1 case of the host batch path
@@ -588,7 +573,7 @@ static void* stream_create(int bits, uint64_t seed)
     if (cudaStreamCreateWithFlags(&h->st, cudaStreamNonBlocking) != cudaSuccess ||
         cudaMalloc(&h->d_state, bits == 32 ? sizeof(Xxh32State) : sizeof(Xxh64State)) != cudaSuccess ||
         cudaHostAlloc(&h->h_out, 8, cudaHostAllocDefault) != cudaSuccess) { fail_cuda(cudaGetLastError(), "stream_create"); delete h; return nullptr; }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     if (bits == 32) launch_xxh32_stream((Xxh32State*)h->d_state, XXH_OP_RESET, (uint32_t)seed, nullptr, 0, h->st);
     else            launch_xxh64_stream((Xxh64State*)h->d_state, XXH_OP_RESET, seed, nullptr, 0, h->st);
     return h;
@@ -597,7 +582,7 @@ static void stream_reset(void* hv, uint64_t seed)
 {
     StreamHandle* h = (StreamHandle*)hv; if (!h) return;
     cudaSetDevice(h->device);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     if (h->bits == 32) launch_xxh32_stream((Xxh32State*)h->d_state, XXH_OP_RESET, (uint32_t)seed, nullptr, 0, h->st);
     else               launch_xxh64_stream((Xxh64State*)h->d_state, XXH_OP_RESET, seed, nullptr, 0, h->st);
 }
@@ -606,15 +591,10 @@ static int stream_update(void* hv, const void* input, size_t len)
     StreamHandle* h = (StreamHandle*)hv; if (!h) return fail_arg("null state");
     if (len == 0) return 0;
     CK(cudaSetDevice(h->device));
-    if (len > h->buf_cap) {
-        CK(cudaStreamSynchronize(h->st));
-        if (h->d_buf) CK(cudaFree(h->d_buf));
-        h->d_buf = nullptr; h->buf_cap = 0;
-        size_t cap = len + (len >> 1) + 4096;
-        CK(cudaMalloc(&h->d_buf, cap)); h->buf_cap = cap;
-    }
+    if (len > h->buf_cap) CK(cudaStreamSynchronize(h->st));
+    const int rc = reserve_device(h->d_buf, h->buf_cap, len, 1); if (rc) return rc;       // half again: update sizes often keep rising
     CK(cudaMemcpyAsync(h->d_buf, input, len, cudaMemcpyHostToDevice, h->st));
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     if (h->bits == 32) CK(launch_xxh32_stream((Xxh32State*)h->d_state, XXH_OP_UPDATE, 0, h->d_buf, len, h->st));
     else               CK(launch_xxh64_stream((Xxh64State*)h->d_state, XXH_OP_UPDATE, 0, h->d_buf, len, h->st));
     CK(cudaStreamSynchronize(h->st));          // the caller may reuse `input` as soon as we return
@@ -625,7 +605,7 @@ static uint64_t stream_digest(void* hv)
     tl_status = 0;
     StreamHandle* h = (StreamHandle*)hv; if (!h) { fail_arg("null state"); return 0; }
     cudaSetDevice(h->device);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     if (h->bits == 32) {
         launch_xxh32_stream((Xxh32State*)h->d_state, XXH_OP_DIGEST, 0, nullptr, 0, h->st);
         cudaMemcpyAsync(h->h_out, &((Xxh32State*)h->d_state)->digest, 4, cudaMemcpyDeviceToHost, h->st);
@@ -685,14 +665,14 @@ int b200lz4_decompress_fast_batch_dev(const uint8_t* src_base, const uint64_t* s
 int b200xxh32_batch_dev(const uint8_t* base, const uint64_t* off, const int32_t* len, uint32_t seed, uint32_t* out, size_t n, void* stream)
 {
     int rc = ensure_device(); if (rc) return rc;
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     CK(launch_xxh32(base, off, len, seed, out, n, (cudaStream_t)stream));
     return 0;
 }
 int b200xxh64_batch_dev(const uint8_t* base, const uint64_t* off, const int32_t* len, uint64_t seed, uint64_t* out, size_t n, void* stream)
 {
     int rc = ensure_device(); if (rc) return rc;
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
     CK(launch_xxh64(base, off, len, seed, out, n, (cudaStream_t)stream));
     return 0;
 }
@@ -705,7 +685,7 @@ int b200lz4_compact_dev(const uint8_t* slots, const uint64_t* slot_off, const in
     if (n > 0xFFFFFFFFull) return fail_arg("n");
     if (!total || (n && (!slots || !slot_off || !lens || !out || !out_off))) return fail_arg("null pointer");
     if (n == 0) { CK(cudaMemsetAsync(total, 0, sizeof(uint64_t), (cudaStream_t)stream)); return 0; }
-    g_launches.fetch_add(2, std::memory_order_relaxed);
+    g_launch_count.fetch_add(2, std::memory_order_relaxed);
     CK(launch_compact(slots, slot_off, lens, out, out_off, total, n, (cudaStream_t)stream));
     return 0;
 }
@@ -789,64 +769,46 @@ int b200lz4_compress_fast_compact_host(const uint8_t* src_base, const uint64_t* 
     if (total) *total = 0;
     if (n == 0) return 0;
     if (!src_base || !src_off || !src_len || !dst_base || !out_off || !result) return fail_arg("null pointer");
-    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
-    PipelineGuard guard(c);
+    // stage: each block gets a bound-sized slot in d_dst, launch_compact packs the results into d_aux
+    auto stage = [&](Slot& s, const Chunk& ch) -> int {
+        uint64_t bound_sum = 0;
+        for (size_t k = ch.i0; k < ch.i0 + ch.nb; k++) bound_sum += aligned_compress_bound((uint64_t)(src_len[k] > 0 ? src_len[k] : 0));
+        int rc = slot_reserve(s, ch.s_span + 16, (size_t)bound_sum + 16, ch.nb, (size_t)bound_sum + 16); if (rc) return rc;
+        const size_t s_phase = (size_t)((uintptr_t)(src_base + ch.s_lo) & 15);
+        uint64_t slot_pos = 0;
+        for (size_t k = 0; k < ch.nb; k++) {
+            const uint64_t len = (uint64_t)(src_len[ch.i0 + k] > 0 ? src_len[ch.i0 + k] : 0);
+            s.h.soff()[k] = src_off[ch.i0 + k] - ch.s_lo + s_phase;
+            s.h.doff()[k] = slot_pos;
+            s.h.slen()[k] = src_len[ch.i0 + k];
+            s.h.dcap()[k] = (int32_t)compress_bound(len);
+            slot_pos += aligned_compress_bound(len);
+        }
+        CK(cudaMemcpyAsync(s.d.base, s.h.base, s.h.bytes(), cudaMemcpyHostToDevice, s.st));
+        if (ch.s_span) CK(cudaMemcpyAsync(s.d_src + s_phase, src_base + ch.s_lo, ch.s_span, cudaMemcpyHostToDevice, s.st));
+        BatchArgs a{ s.d_src, s.d.soff(), s.d.slen(), s.d_dst, s.d.doff(), s.d.dcap(), s.d.res(), ch.nb };
+        CK(launch_op(OP_COMPRESS_FAST, a, max_src_len, s.st));
+        g_launch_count.fetch_add(2, std::memory_order_relaxed);
+        CK(launch_compact(s.d_dst, s.d.doff(), s.d.res(), s.d_aux, s.d.out(), s.d.total(), ch.nb, s.st));
+        CK(cudaMemcpyAsync(s.h.base, s.d.base, s.h.bytes(), cudaMemcpyDeviceToHost, s.st));
+        return 0;
+    };
+    // retire: learn the chunk's packed size, start the payload copy at the running offset
     uint64_t running = 0;
-    // retire the slot's chunk: learn its packed size, start the payload copy at the running offset
     auto retire = [&](Slot& s) -> int {
-        if (!s.busy) return 0;
-        CK(cudaEventSynchronize(s.done));
-        const uint64_t tot = *s.h_total();
+        const uint64_t tot = *s.h.total();
         if (running + tot > dst_capacity) return fail_arg("dst_capacity too small for the packed stream");
         if (tot) CK(cudaMemcpyAsync(dst_base + running, s.d_aux, (size_t)tot, cudaMemcpyDeviceToHost, s.st));
         CK(cudaEventRecord(s.drained, s.st)); s.draining = true;
         const size_t nb = s.i1 - s.i0;
-        memcpy(result + s.i0, s.h_res(), nb * sizeof(int32_t));
-        for (size_t k = 0; k < nb; k++) out_off[s.i0 + k] = running + s.h_xoff()[k];
-        running += tot; s.busy = false;
+        memcpy(result + s.i0, s.h.res(), nb * sizeof(int32_t));
+        for (size_t k = 0; k < nb; k++) out_off[s.i0 + k] = running + s.h.out()[k];
+        running += tot;
         return 0;
     };
-    size_t i0 = 0; int cur = 0;
-    while (i0 < n) {
-        const uint64_t s_lo = src_off[i0]; uint64_t s_hi = s_lo, bound_sum = 0; size_t i1 = i0;
-        while (i1 < n && i1 - i0 < CHUNK_BLOCKS) {
-            if (src_off[i1] < s_lo) return fail_arg("blocks must ascend");
-            const uint64_t len = (uint64_t)(src_len[i1] > 0 ? src_len[i1] : 0);
-            const uint64_t se = src_off[i1] + len, ns = se > s_hi ? se : s_hi;
-            if (i1 > i0 && ns - s_lo > CHUNK_SPAN) break;
-            s_hi = ns; bound_sum += ((len + len / 255 + 16) + 15) & ~uint64_t(15); i1++;
-        }
-        const size_t nb = i1 - i0, s_span = (size_t)(s_hi - s_lo);
-        Slot& s = c->slot[cur];
-        rc = retire(s); if (rc) return rc;
-        rc = slot_reserve(s, s_span + 16, (size_t)bound_sum + 16, nb, (size_t)bound_sum + 16); if (rc) return rc;
-        const size_t s_phase = (size_t)((uintptr_t)(src_base + s_lo) & 15);
-        uint64_t slot_pos = 0;
-        for (size_t k = 0; k < nb; k++) {
-            const uint64_t len = (uint64_t)(src_len[i0 + k] > 0 ? src_len[i0 + k] : 0);
-            const uint64_t bnd = len + len / 255 + 16;
-            s.h_soff()[k] = src_off[i0 + k] - s_lo + s_phase;
-            s.h_doff()[k] = slot_pos;
-            s.h_slen()[k] = src_len[i0 + k];
-            s.h_dcap()[k] = (int32_t)bnd;
-            slot_pos += (bnd + 15) & ~uint64_t(15);
-        }
-        CK(cudaMemcpyAsync(s.d_desc, s.h_desc, Slot::desc_bytes(s.desc_blocks), cudaMemcpyHostToDevice, s.st));
-        if (s_span) CK(cudaMemcpyAsync(s.d_src + s_phase, src_base + s_lo, s_span, cudaMemcpyHostToDevice, s.st));
-        BatchArgs a{ s.d_src, s.d_soff(), s.d_slen(), s.d_dst, s.d_doff(), s.d_dcap(), s.d_res(), nb };
-        CK(launch_op(OP_COMPRESS_FAST, a, max_src_len, s.st));
-        g_launches.fetch_add(2, std::memory_order_relaxed);
-        CK(launch_compact(s.d_dst, s.d_doff(), s.d_res(), s.d_aux, s.d_xoff(), s.d_total(), nb, s.st));
-        CK(cudaMemcpyAsync(s.h_desc, s.d_desc, Slot::desc_bytes(s.desc_blocks), cudaMemcpyDeviceToHost, s.st));
-        CK(cudaEventRecord(s.done, s.st));
-        s.busy = true; s.i0 = i0; s.i1 = i1;
-        i0 = i1; cur = (cur + 1) % NSLOTS;
-    }
-    for (int k = 0; k < NSLOTS; k++) { rc = retire(c->slot[(cur + k) % NSLOTS]); if (rc) return rc; }
-    for (int k = 0; k < NSLOTS; k++) { Slot& s = c->slot[k]; if (s.draining) { CK(cudaEventSynchronize(s.drained)); s.draining = false; } }
-    if (total) *total = running;
-    guard.completed = true;
-    return 0;
+    const int rc = run_pipeline(n, src_off, src_len, nullptr, nullptr, "blocks must ascend", stage, retire);
+    if (!rc && total) *total = running;
+    return rc;
 }
 
 int b200lz4_compress_fast_batch_host_multi(const uint8_t* src_base, const uint64_t* src_off, const int32_t* src_len,
@@ -880,7 +842,7 @@ int b200lz4_compress_fast_compact_host_multi(const uint8_t* src_base, const uint
         uint64_t acc = 0; int g = 0;
         for (size_t i = 0; i <= n; i++) {
             while (g <= ndev && i == n * (size_t)g / (size_t)ndev) base[(size_t)g++] = acc;
-            if (i < n) { const uint64_t len = (uint64_t)(src_len[i] > 0 ? src_len[i] : 0); acc += ((len + len / 255 + 16) + 15) & ~uint64_t(15); }
+            if (i < n) acc += aligned_compress_bound((uint64_t)(src_len[i] > 0 ? src_len[i] : 0));
         }
         if (acc > dst_capacity) return fail_arg("dst_capacity must hold the aligned bounds of all blocks");
     }
@@ -914,7 +876,7 @@ int b200xxh64_batch_host_multi(const uint8_t* base, const uint64_t* off, const i
 }
 
 int b200lz4_context_count(void) { return g_contexts.load(std::memory_order_relaxed); }
-uint64_t b200lz4_launch_count(void) { return g_launches.load(std::memory_order_relaxed) + g_launch_count.load(std::memory_order_relaxed); }
-void     b200lz4_launch_count_reset(void) { g_launches.store(0, std::memory_order_relaxed); g_launch_count.store(0, std::memory_order_relaxed); }
+uint64_t b200lz4_launch_count(void) { return g_launch_count.load(std::memory_order_relaxed); }
+void     b200lz4_launch_count_reset(void) { g_launch_count.store(0, std::memory_order_relaxed); }
 
 } // extern "C"

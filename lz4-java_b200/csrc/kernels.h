@@ -54,6 +54,14 @@ cudaError_t launch_xxh64_long(const uint8_t* base, const uint64_t* off, const in
 cudaError_t launch_compact(const uint8_t* slots, const uint64_t* slot_off, const int32_t* lens,
                            uint8_t* out, uint64_t* out_off, uint64_t* total, size_t n, cudaStream_t st);
 
-extern std::atomic<unsigned long long> g_launch_count;      // launches made outside capi.cu (frame / container calls, any thread)
+// Average buffer length from which the hash batches give each buffer a whole warp (launch_xxh*_long) instead of a lane.
+static constexpr uint64_t XXH_LONG_AVG = 32768;
+
+// LZ4_compressBound(len) (lz4.h:212) without its range check, and the room one block takes in a packed compress
+// staging area: that bound rounded up to 16 bytes.
+static inline uint64_t compress_bound(uint64_t len) { return len + len / 255 + 16; }
+static inline uint64_t aligned_compress_bound(uint64_t len) { return (compress_bound(len) + 15) & ~uint64_t(15); }
+
+extern std::atomic<unsigned long long> g_launch_count;      // every kernel launch the library makes (any thread): b200lz4_launch_count()
 
 } // namespace b200

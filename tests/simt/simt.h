@@ -50,7 +50,9 @@ inline void release(void* p) { if (p) std::free(((void**)p)[-1]); }
 }
 template <class T> static inline cudaError_t cudaMalloc(T** p, size_t n) { *p = (T*)simt_rt::alloc(n); return *p ? cudaSuccess : 2; }
 static inline cudaError_t cudaFree(void* p) { simt_rt::release(p); return cudaSuccess; }
-template <class T> static inline cudaError_t cudaHostAlloc(T** p, size_t n, unsigned) { *p = (T*)simt_rt::alloc(n); return *p ? cudaSuccess : 2; }
+// SIMT_FAIL_HOST_ALLOC set: every pinned allocation fails, as a real one can when the host is short of pinnable memory
+template <class T> static inline cudaError_t cudaHostAlloc(T** p, size_t n, unsigned)
+{ *p = std::getenv("SIMT_FAIL_HOST_ALLOC") ? nullptr : (T*)simt_rt::alloc(n); return *p ? cudaSuccess : 2; }
 static inline cudaError_t cudaFreeHost(void* p) { simt_rt::release(p); return cudaSuccess; }
 static inline cudaError_t cudaHostRegister(void*, size_t, unsigned) { return cudaSuccess; }
 static inline cudaError_t cudaHostUnregister(void*) { return cudaSuccess; }

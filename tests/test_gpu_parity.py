@@ -332,7 +332,7 @@ def test_compact_host(b200, checker):
         pos += int(olen[k])
 
 
-def test_failed_pipeline_call_leaves_nothing_in_flight(b200):
+def test_failed_pipeline_call_leaves_nothing_in_flight(b200, checker):
     """A host-buffer call that fails after some chunks were queued (here: `dst_capacity too small for the packed stream`,
     found when the FIRST chunk retires while the next two are in flight) must drain them: the next call on the same
     thread would otherwise retire the stale chunks into its own result / offset arrays.  Three chunks are needed: chunks
@@ -369,6 +369,15 @@ def test_failed_pipeline_call_leaves_nothing_in_flight(b200):
         b200.batch.compress_fast_batch_host(src, soff, slen, comp, bad, ccap, max_src_len=65536)
     clen = b200.batch.compress_fast_batch_host(src[:7 * bl], soff[:7], slen[:7], comp, coff[:7], ccap[:7], max_src_len=65536)
     assert (clen == cl).all() and (comp[:7 * cl].reshape(7, cl)[:, hdr:] == src[:7 * bl].reshape(7, bl)).all()
+    # the hash path after its own argument error (a buffer out of order, found at the third chunk).  The next call hashes
+    # 7 buffers into the head of a longer array: a chunk left in flight would be retired into the entries behind them.
+    hbad = soff.copy(); hbad[2 * per_chunk + 50] = 0
+    with pytest.raises(b200.B200Error, match="ascend"):
+        b200.batch.xxh64_batch_host(src, hbad, slen, 1)
+    h = np.full(n, 0x5555, dtype=np.uint64)
+    assert b200._native.lib().b200xxh64_batch_host(src.ctypes.data, soff.ctypes.data, slen.ctypes.data, 2, h.ctypes.data, 7) == 0
+    assert [int(x) for x in h[:7]] == [checker.xxh64(src[k * bl:(k + 1) * bl], 2) for k in range(7)]
+    assert (h[7:] == 0x5555).all()
 
 
 def test_xxhash_batches(b200, checker):

@@ -339,7 +339,13 @@ def test_compaction_scan_and_gather(msim):
 
 
 # ---------------------------------------------------------------------------------------------- the host layer too
-def test_host_layer_on_the_emulator_library():
+@pytest.fixture(scope="module")
+def sim_library():
+    subprocess.run(["bash", os.path.join(HERE, "simt", "build_sim_library.sh")], check=True, capture_output=True)
+    return os.path.join(HERE, "simt", "_build", "libb200lz4_sim.so")
+
+
+def test_host_layer_on_the_emulator_library(sim_library):
     """tests/simt/build_sim_library.sh builds the WHOLE library for the emulator (capi.cu / frame.cu / containers.cu
     unchanged over a stand-in CUDA runtime); a few of the GPU parity tests then run against it in a subprocess (the
     product loader of this process is left alone): the batch pipeline with bounce buffers and compaction, the
@@ -347,10 +353,41 @@ def test_host_layer_on_the_emulator_library():
     fails half way, the JNI shim, the range-sharded multi-GPU calls and the device-side stitch over three pretend devices (SIMT_DEVICES), frames written with flush().  The full file takes ~20 minutes this way
     (see tests/simt/README.md); this is the one-minute slice."""
     import sys
-    subprocess.run(["bash", os.path.join(HERE, "simt", "build_sim_library.sh")], check=True, capture_output=True)
     # 1 MiB pipeline chunks: the 40-block batches of these tests then cross chunk boundaries (all three stream slots in use)
-    env = dict(os.environ, B200LZ4_TEST_SO=os.path.join(HERE, "simt", "_build", "libb200lz4_sim.so"), B200LZ4_CHUNK_MB="1", SIMT_DEVICES="3")
+    env = dict(os.environ, B200LZ4_TEST_SO=sim_library, B200LZ4_CHUNK_MB="1", SIMT_DEVICES="3")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(HERE, "test_gpu_parity.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
                         "-W", "ignore::DeprecationWarning", "-k", "factory_api or compact_host or xxhash_streaming or self_roundtrip or failed_pipeline or contexts_are_reused or jni_shim or multi_gpu_range or written_with_flush or device_side_compaction or stream_order"],
                        env=env, cwd=ROOT, capture_output=True, text=True)
     assert r.returncode == 0 and "11 passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+
+
+_FAILED_ALLOC = r"""
+import ctypes, os, sys
+import numpy as np
+lib = ctypes.CDLL(sys.argv[1])
+lib.b200xxh64_batch_host.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_uint64, ctypes.c_void_p, ctypes.c_size_t]
+lib.b200lz4_last_error.restype = ctypes.c_char_p
+buf = np.random.default_rng(5).integers(0, 256, 100 * 64, dtype=np.uint8)
+off, ln = np.arange(100, dtype=np.uint64) * np.uint64(64), np.full(100, 64, dtype=np.int32)
+def hash_(n):
+    out = np.zeros(n, dtype=np.uint64)
+    return lib.b200xxh64_batch_host(buf.ctypes.data, off.ctypes.data, ln.ctypes.data, 0, out.ctypes.data, n), out
+rc, first = hash_(10)
+assert rc == 0, rc
+os.environ["SIMT_FAIL_HOST_ALLOC"] = "1"
+rc, _ = hash_(100)                          # the slot's descriptor arrays must grow: the pinned half fails
+del os.environ["SIMT_FAIL_HOST_ALLOC"]
+assert rc < 0 and b"cudaHostAlloc" in lib.b200lz4_last_error(), (rc, lib.b200lz4_last_error())
+rc, again = hash_(10)
+assert rc == 0 and (again == first).all(), rc
+print("ok")
+"""
+
+
+def test_failed_staging_allocation_leaves_the_slot_usable(sim_library):
+    """A pipeline slot whose staging cannot grow (the pinned allocation fails after the old buffer was freed) fails that
+    call with a CUDA error, and the next, smaller call on the thread allocates again instead of staging through the
+    freed buffer.  Runs in a subprocess: the regression is a crash."""
+    import sys
+    r = subprocess.run([sys.executable, "-c", _FAILED_ALLOC, sim_library], capture_output=True, text=True)
+    assert r.returncode == 0 and r.stdout.strip() == "ok", (r.returncode, r.stdout[-2000:] + r.stderr[-2000:])
