@@ -30,6 +30,7 @@
 #ifndef B200_WIDE_WARPS
 #define B200_WIDE_WARPS 3
 #endif
+// (The tag width of that kernel, B200_WIDE_TAG_BITS, is set in lz4_compress_wide.cuh.)
 
 namespace b200 {
 
@@ -237,18 +238,33 @@ static cudaError_t launch_long(const BatchArgs& a, cudaStream_t st)
 
 
 #ifndef B200_HOST_SIM
-template <int HASH_LOG, int NB, int NW>
+#ifdef B200_WIDE_TRACE
+// -DB200_WIDE_TRACE builds only: the per-role cycle counts of the last launch (lz4_compress_wide.cuh), first `rows` rows,
+// and the CTAs per SM the runtime reports for the kernel that launch used
+static int g_wide_ctas_per_sm = 0;
+extern "C" int b200lz4_wide_trace_read(unsigned long long* host, int rows)
+{
+    if (rows < 0 || rows > WIDE_TRACE_ROWS) return -1;
+    return cudaMemcpyFromSymbol(host, g_wide_trace, size_t(rows) * WT_N * sizeof(unsigned long long)) == cudaSuccess ? WT_N : -1;
+}
+extern "C" int b200lz4_wide_trace_ctas_per_sm() { return g_wide_ctas_per_sm; }
+#endif
+
+template <int HASH_LOG, int NB, int NW, int TAG_BITS>
 static cudaError_t launch_wide(const BatchArgs& a, cudaStream_t st)
 {
     constexpr int S = 2;                                                     // sub-rounds of 128 positions per chunk
-    using LY = WideLayout<S, NB, NW>;
+    using LY = WideLayout<S, NB, NW, TAG_BITS>;
     const size_t smem = LY::smem(HASH_LOG);
     constexpr int FIT = 233472 / (int(LY::smem(HASH_LOG)) + 1024);          // CTAs per SM that shared memory allows
     constexpr int MINB = FIT < 16 ? FIT : 16;
-    auto k = lz4_compress_wide_kernel<HASH_LOG, S, NB, NW, MINB>;
+    auto k = lz4_compress_wide_kernel<HASH_LOG, S, NB, NW, MINB, TAG_BITS>;
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+#ifdef B200_WIDE_TRACE
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g_wide_ctas_per_sm, k, 32 * NW, smem);
+#endif
     k<<<(unsigned)a.n, 32 * NW, smem, st>>>(a.src_base, a.src_off, a.src_len, a.dst_base, a.dst_off, a.dst_cap, a.result, (uint32_t)a.n);
     return cudaGetLastError();
 }
@@ -257,7 +273,7 @@ static cudaError_t launch_wide(const BatchArgs& a, cudaStream_t st)
 cudaError_t launch_compress_fast(const BatchArgs& a, int max_src_len, cudaStream_t st)
 {
     if (a.n == 0) return cudaSuccess;
-    if (max_src_len > 0 && max_src_len <= 65536) return launch_wide<13, 2, B200_WIDE_WARPS>(a, st);   // 8192 x u16: lz4.c:1353
+    if (max_src_len > 0 && max_src_len <= 65536) return launch_wide<13, 2, B200_WIDE_WARPS, B200_WIDE_TAG_BITS>(a, st);   // 8192 x u16: lz4.c:1353
     return launch_long<12, false>(a, st);                  // 4096 x u32 = 16 KiB, the reference's byU32 table (lz4.c:1356)
 }
 #endif

@@ -12,7 +12,8 @@
 // hits speculatively (the round-1 parser: 14 loads per hit, 32 hits per round) spends most of its instructions on hits the
 // greedy chain then skips.  Here
 //   warp L  walks the block in chunks of 128*S positions, S sub-rounds of 128 in order: probe 4 positions per lane,
-//           barrier, insert, then verify every candidate against EIGHT bytes (three aligned words per side).  Per position
+//           barrier, insert, then verify every candidate whose hash tag matches (TAG_BITS below) against EIGHT bytes (three
+//           aligned words of the position, one aligned 16-byte load of the candidate, two when they straddle it).  Per position
 //           it publishes a u16 distance and a byte: the verified length (4..8) and how far the next hit behind the match is; per
 //           chunk a hit mask.
 //   warp P  walks the chain on warp-uniform values: two shared-memory loads per sequence give distance, length and the
@@ -31,6 +32,14 @@
 #include "lz4_emit.cuh"
 #include <type_traits>
 
+// Hash-tag bits per table slot (0, 1, 2, 4 or 8; 0 = no tags), the default of the kernel's TAG_BITS.  Every width emits the
+// same bytes; wider tags skip more verify loads but leave room for fewer CTAs per SM (shared memory: 12, 11, 10, 9, 8; the
+// runtime reports 9 for the untagged kernel).  8 measured fastest on the bench corpus (DESIGN.md §4).  A build-time choice
+// (tools/build_variants.sh), not a runtime switch.
+#ifndef B200_WIDE_TAG_BITS
+#define B200_WIDE_TAG_BITS 8
+#endif
+
 namespace b200 {
 
 #ifdef B200_HOST_SIM
@@ -38,7 +47,8 @@ __device__ __forceinline__ void wide_bar_arrive(int id) { simt::bar_arrive(id, 6
 __device__ __forceinline__ void wide_bar_wait(int id) { simt::bar_sync(id, 64); }
 __device__ __forceinline__ uint32_t ldg_u32(const uint32_t* p) { return *p; }
 __device__ __forceinline__ void ldg_pair(const uint32_t* base, uint32_t idx, uint32_t& lo, uint32_t& hi) { lo = base[idx]; hi = base[idx + 1]; }
-__device__ __forceinline__ uint2 ldg_u64(const uint2* p) { return *p; }
+__device__ __forceinline__ uint4 ldg_u128(const uint4* p) { return *p; }
+__device__ __forceinline__ void shared_xor(uint32_t* p, uint32_t v) { *p ^= v; }     // (the emulator runs one lane at a time)
 #else
 // (Immediate barrier ids, so ptxas reserves only the barriers in use and not all 16.)
 #define B200_WBAR_CASE(OP, N) case N: asm volatile(OP " " #N ", 64;" ::: "memory"); break;
@@ -53,7 +63,8 @@ __device__ __forceinline__ void wide_bar_wait(int id)
                   B200_WBAR_CASE("bar.sync", 4) B200_WBAR_CASE("bar.sync", 5) default: asm volatile("bar.sync 6, 64;" ::: "memory"); }
 }
 __device__ __forceinline__ uint32_t ldg_u32(const uint32_t* p) { return __ldg(p); }      // the input is read-only for the kernel
-__device__ __forceinline__ uint2 ldg_u64(const uint2* p) { return __ldg(p); }
+__device__ __forceinline__ uint4 ldg_u128(const uint4* p) { return __ldg(p); }
+__device__ __forceinline__ void shared_xor(uint32_t* p, uint32_t v) { atomicXor(p, v); }
 // words idx and idx + 1 of a read-only array: one 32x32+64 multiply-add for the address, two loads off it
 __device__ __forceinline__ void ldg_pair(const uint32_t* base, uint32_t idx, uint32_t& lo, uint32_t& hi)
 {
@@ -64,32 +75,64 @@ __device__ __forceinline__ void ldg_pair(const uint32_t* base, uint32_t idx, uin
 }
 #endif
 
-template <int S, int NB, int NW>
+// Per-role cycle accounting (builds with -DB200_WIDE_TRACE only; tools/compress_roles.py reads it): every 64th CTA, lane 0
+// of each warp adds up the clock64 cycles its warp spends in the marked waits and calls and writes them, with its total, to
+// row blockIdx / 64 of g_wide_trace.  Without the flag the macros are empty and the kernel is the same code.
+#ifdef B200_WIDE_TRACE
+enum { WT_L_TOTAL, WT_L_FREE, WT_E_TOTAL, WT_E_REC_FULL, WT_P_TOTAL, WT_P_FULL, WT_P_REC_FREE, WT_P_EXTEND, WT_P_SEARCH,
+       WT_SEQUENCES, WT_EXTENDS, WT_SEARCHES, WT_N };           // (tools/compress_roles.py reads the rows in this order)
+constexpr int WIDE_TRACE_EVERY = 64, WIDE_TRACE_ROWS = 16384;
+__device__ unsigned long long g_wide_trace[WIDE_TRACE_ROWS][WT_N];
+#define WT_BEGIN unsigned long long wt[WT_N] = {}; const long long wt_start = clock64()
+#define WT_TIME(slot, ...) do { const long long t_ = clock64(); __VA_ARGS__; wt[slot] += clock64() - t_; } while (0)
+#define WT_COUNT(slot) (wt[slot] += 1)
+#define WT_END(total, lo, hi) do {                                                                                   \
+        wt[total] = clock64() - wt_start;                                                                           \
+        if (lane == 0 && b % WIDE_TRACE_EVERY == 0 && b / WIDE_TRACE_EVERY < WIDE_TRACE_ROWS) {                     \
+            g_wide_trace[b / WIDE_TRACE_EVERY][total] = wt[total];                                                 \
+            for (int i_ = lo; i_ < hi; i_++) g_wide_trace[b / WIDE_TRACE_EVERY][i_] = wt[i_];                      \
+        } } while (0)
+#else
+#define WT_BEGIN
+#define WT_TIME(slot, ...) do { __VA_ARGS__; } while (0)
+#define WT_COUNT(slot)
+#define WT_END(total, lo, hi)
+#endif
+
+template <int S, int NB, int NW, int TAG_BITS>
 struct WideLayout {
     static constexpr int CH = 128 * S;                 // positions per chunk
     static constexpr int MW = CH / 32;                 // mask words per chunk
     static constexpr int BUF_BYTES = CH * 3 + MW * 4;  // u16 distances + u8 jump/length codes + hit mask
     static constexpr int REC_BYTES = 32 * 8 + 16;      // one batch of sequence records + its header
-    static constexpr size_t smem(int hash_log) { return (size_t(2) << hash_log) + size_t(NB) * BUF_BYTES + REC_BYTES; }
+    static constexpr size_t tag_bytes(int hash_log) { return (size_t(TAG_BITS) << hash_log) / 8; }
+    static constexpr size_t smem(int hash_log)
+    { return (size_t(2) << hash_log) + tag_bytes(hash_log) + size_t(NB) * BUF_BYTES + REC_BYTES; }
 };
 
-template <int HASH_LOG, int S, int NB, int NW, int MINB>
+// TAG_BITS > 0: next to every table slot the lookup warp keeps TAG_BITS more bits of the hash of the position stored
+// there (the bits of the same product just below the slot index).  A candidate whose tag differs from the probing
+// position's own cannot share its first 4 bytes, so its verify loads are not issued.  TAG_BITS = 0 is the plain table.
+template <int HASH_LOG, int S, int NB, int NW, int MINB, int TAG_BITS = B200_WIDE_TAG_BITS>
 __global__ void __launch_bounds__(32 * NW, MINB)
 lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off,
                          const int32_t* __restrict__ src_len,
                          uint8_t* __restrict__ dst_base, const uint64_t* __restrict__ dst_off,
                          const int32_t* __restrict__ dst_cap, int32_t* __restrict__ result, uint32_t nblocks)
 {
-    using LY = WideLayout<S, NB, NW>;
+    using LY = WideLayout<S, NB, NW, TAG_BITS>;
     constexpr int CH = LY::CH, MW = LY::MW;
     constexpr int TABLE_BYTES = 2 << HASH_LOG;
+    constexpr int TAG_BYTES = int(LY::tag_bytes(HASH_LOG));
     constexpr int BAR_FULL = 1, BAR_FREE = 1 + NB, BAR_REC_FULL = 1 + 2 * NB, BAR_REC_FREE = 2 + 2 * NB;
     constexpr int REC_LAST = 0x100;                        // batch header flag: no batch follows
     static_assert(NW == 2 || NW == 3, "two or three warps");
     static_assert(2 * NB + (NW == 3 ? 2 : 0) <= 6, "named barrier ids 1..6");
+    static_assert(TAG_BITS == 0 || TAG_BITS == 1 || TAG_BITS == 2 || TAG_BITS == 4 || TAG_BITS == 8, "tag widths 0, 1, 2, 4, 8");
     B200_DYN_SMEM(smem_raw, 128);
     uint16_t* table = reinterpret_cast<uint16_t*>(smem_raw);
-    uint8_t* bufs = smem_raw + TABLE_BYTES;
+    uint8_t* tags = smem_raw + TABLE_BYTES;               // TAG_BITS per slot, slot h at bit TAG_BITS * h
+    uint8_t* bufs = smem_raw + TABLE_BYTES + TAG_BYTES;
     auto dist_of = [&](int buf) { return reinterpret_cast<uint16_t*>(bufs + buf * LY::BUF_BYTES); };
     auto flen_of = [&](int buf) { return bufs + buf * LY::BUF_BYTES + CH * 2; };
     auto hmask_of = [&](int buf) { return reinterpret_cast<uint32_t*>(bufs + buf * LY::BUF_BYTES + CH * 3); };
@@ -107,12 +150,13 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
 
     if (n < 0 || n >= 65536 + 11 || cap < 0) { if (threadIdx.x == 0) result[b] = 0; return; }     // lz4.c:1324, 973; no room at all
     if (n == 0) { if (threadIdx.x == 0) { if (cap >= 1) dst[0] = 0; result[b] = cap >= 1 ? 1 : 0; } return; }   // lz4.c:1325-1336
+    WT_BEGIN;
 
     // aligned-word view of the block: byte a of the view is position a - ph
     const uint32_t ph = uint32_t(reinterpret_cast<uintptr_t>(src)) & 3u;
     const uint32_t* __restrict__ wsrc = reinterpret_cast<const uint32_t*>(reinterpret_cast<uintptr_t>(src) - ph);
-    const uint32_t ph8 = uint32_t(reinterpret_cast<uintptr_t>(src)) & 7u;                 // ... and the same in 8-byte words
-    const uint2* __restrict__ qsrc = reinterpret_cast<const uint2*>(reinterpret_cast<uintptr_t>(src) - ph8);
+    const uint32_t ph16 = uint32_t(reinterpret_cast<uintptr_t>(src)) & 15u;               // ... and the same in 16-byte words
+    const uint4* __restrict__ osrc = reinterpret_cast<const uint4*>(reinterpret_cast<uintptr_t>(src) - ph16);
     const int mflimit = n - 12, matchlimit = n - 5;        // lz4.c:243-244
     const int nchunks = mflimit >= 0 ? (mflimit + int(ph)) / CH + 1 : 0;     // n < 13: all literals (lz4.c:981)
     auto ld4 = [&](int pos) -> uint32_t {                  // the 4 bytes at position pos
@@ -124,7 +168,15 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
 
     if (role == 0) {
         // ================================================================== warp L: probe, insert, verify 8 bytes
+        constexpr uint32_t TMASK = (1u << TAG_BITS) - 1u;
+        auto tag_of = [](uint32_t prod) { return (prod >> (32 - HASH_LOG - TAG_BITS)) & TMASK; };
+        uint32_t* tagw = reinterpret_cast<uint32_t*>(tags);
+        auto tag_get = [&](uint32_t h) { return (tagw[(TAG_BITS * h) >> 5] >> ((TAG_BITS * h) & 31u)) & TMASK; };
+        // An untouched slot holds position 0, so its tag starts as position 0's: the probes of the first sub-round run before
+        // position 0 is inserted and may still find it (bytes 0..3 == p..p+3 at the start of a run).
+        const uint32_t tag0 = (TAG_BITS && nchunks) ? tag_of(ld4(0) * 2654435761u) * (0xFFFFFFFFu / max(TMASK, 1u)) : 0u;
         for (int i = lane; i < TABLE_BYTES / 16; i += 32) reinterpret_cast<uint4*>(table)[i] = make_uint4(0, 0, 0, 0);
+        for (int i = lane; i < TAG_BYTES / 16; i += 32) reinterpret_cast<uint4*>(tags)[i] = make_uint4(tag0, tag0, tag0, tag0);
         __syncwarp();
         // One chunk.  EDGE = false is the body for chunks whose positions are all inside [1, mflimit): there every position is
         // valid, every table entry is a position inserted earlier (< p) and 8 bytes fit below matchlimit, so no validity
@@ -135,6 +187,7 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
             const int cp0 = CH * c - int(ph);
             // ---- phase 1, sub-round by sub-round: probe all 128 positions, then insert all 128
             uint32_t w0[S], w1[S], w2[S]; int cand[S][4];
+            uint32_t tok = TAG_BITS ? 0u : 0xFFFFFFFFu;    // bit 4s + j: the candidate's tag equals the position's own
             #pragma unroll
             for (int s = 0; s < S; s++) {
                 const int p0 = cp0 + 128 * s + 4 * lane;
@@ -146,11 +199,18 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
             for (int s = 0; s < S; s++) {
                 const int p0 = cp0 + 128 * s + 4 * lane;
                 uint32_t h[4];
+                [[maybe_unused]] uint32_t t[4], ct[4];                                           // (TAG_BITS > 0)
                 #pragma unroll
                 for (int j = 0; j < 4; j++) {
                     const uint32_t sq = j ? __funnelshift_r(w0[s], w1[s], 8 * j) : w0[s];
-                    h[j] = (sq * 2654435761u) >> (32 - HASH_LOG);
+                    const uint32_t prod = sq * 2654435761u;
+                    h[j] = prod >> (32 - HASH_LOG);
                     cand[s][j] = table[h[j]];
+                    if constexpr (TAG_BITS > 0) {
+                        t[j] = tag_of(prod);
+                        ct[j] = tag_get(h[j]);
+                        tok |= uint32_t(ct[j] == t[j]) << (4 * s + j);
+                    }
                 }
                 __syncwarp();  // every probe of the sub-round precedes every insert (same-slot stores: any winner is a valid position)
                 #pragma unroll
@@ -159,9 +219,24 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
                     if (!EDGE || (p >= 0 && p <= mflimit)) table[h[j]] = uint16_t(p);
                 }
                 __syncwarp();  // ... and every insert precedes the next sub-round's probes
+                if constexpr (TAG_BITS > 0) {
+                    // Only the lane whose position won the slot writes its tag, so a slot never pairs one lane's position with
+                    // another's tag, however the same-slot stores above were ordered.  Nobody else writes those tag bits in this
+                    // sub-round, so they still hold ct (what this lane probed): one XOR of ct ^ t sets them, and lanes that share
+                    // a word touch disjoint bits.
+                    #pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        const int p = p0 + j;
+                        if ((!EDGE || (p >= 0 && p <= mflimit)) && table[h[j]] == uint16_t(p)) {
+                            if constexpr (TAG_BITS == 8) tags[h[j]] = uint8_t(t[j]);
+                            else if (ct[j] != t[j]) shared_xor(&tagw[(TAG_BITS * h[j]) >> 5], (ct[j] ^ t[j]) << ((TAG_BITS * h[j]) & 31u));
+                        }
+                    }
+                    __syncwarp();  // every tag is written before the next sub-round's probes
+                }
             }
             // ---- phase 2: all candidates of the chunk are verified with independent loads (one L2 round trip per chunk)
-            if (c >= NB) wide_bar_wait(BAR_FREE + buf);    // warp P is done with this buffer's previous tenant
+            if (c >= NB) WT_TIME(WT_L_FREE, wide_bar_wait(BAR_FREE + buf));    // warp P is done with this buffer's previous tenant
             uint16_t* ds = dist_of(buf);
             uint8_t* fls = flen_of(buf);
             uint32_t* hm = hmask_of(buf);
@@ -175,11 +250,17 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
                     const int p = p0 + j;
                     const uint32_t sq = j ? __funnelshift_r(w0[s], w1[s], 8 * j) : w0[s];        // bytes p .. p+3
                     const uint32_t sn = j ? __funnelshift_r(w1[s], w2[s], 8 * j) : w1[s];        // bytes p+4 .. p+7
-                    const bool plaus = !EDGE || (p >= 0 && p <= mflimit && cand[s][j] < p);
-                    // the candidate's 8 bytes sit in two aligned 8-byte words: two scattered loads instead of three
-                    const uint32_t a = uint32_t(plaus ? cand[s][j] : 0) + ph8;                   // (position 0 is always readable)
-                    const uint2* w = qsrc + (a >> 3);
-                    const uint2 q0 = ldg_u64(w), q1 = ldg_u64(w + 1);
+                    const bool plaus = (!EDGE || (p >= 0 && p <= mflimit && cand[s][j] < p)) && ((tok >> (4 * s + j)) & 1u);
+                    // The candidate's 8 bytes: its aligned 16-byte word, and the next one only when they straddle it.  No
+                    // load for an implausible candidate; what is computed from the zeros then is never read (no hit bit).
+                    const uint32_t a = uint32_t(cand[s][j]) + ph16;
+                    const uint4* w = osrc + (a >> 4);
+                    uint4 v = make_uint4(0, 0, 0, 0), v2 = make_uint4(0, 0, 0, 0);
+                    if (plaus) v = ldg_u128(w);
+                    if (plaus && (a & 15u) > 8u) v2 = ldg_u128(w + 1);
+                    const bool h8 = (a & 8u) != 0;                                               // the two aligned 8-byte words
+                    const uint2 q0 = h8 ? make_uint2(v.z, v.w) : make_uint2(v.x, v.y);
+                    const uint2 q1 = h8 ? make_uint2(v2.x, v2.y) : make_uint2(v.z, v.w);
                     const bool up = (a & 4u) != 0;
                     const uint32_t c0 = up ? q0.y : q0.x, c1 = up ? q1.x : q0.y, c2 = up ? q1.y : q1.x;
                     const uint32_t x = __funnelshift_r(c0, c1, a << 3) ^ sq;
@@ -228,6 +309,7 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
             if (c > 0 && cp0 + CH - 1 < mflimit) lookup(c, std::false_type{});
             else lookup(c, std::true_type{});
         }
+        WT_END(WT_L_TOTAL, WT_L_FREE, WT_L_FREE + 1);
         return;
     }
 
@@ -342,11 +424,12 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
     if (NW == 3 && role == 2) {
         // ================================================================== warp E: lay out batches of 32 sequences
         for (;;) {
-            wide_bar_wait(BAR_REC_FULL);
+            WT_TIME(WT_E_REC_FULL, wide_bar_wait(BAR_REC_FULL));
             const int hdr = s_hdr[0], fin = s_hdr[1];
             layout_batch(hdr & 0xFF);
             if (hdr & REC_LAST) { finish(fin); break; }
         }
+        WT_END(WT_E_TOTAL, WT_E_REC_FULL, WT_E_REC_FULL + 1);
         return;
     }
 
@@ -355,13 +438,13 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
         if (NW == 2) { __syncwarp(); layout_batch(k); k = 0; __syncwarp(); return; }
         if (lane == 0) { s_hdr[0] = k | (last ? REC_LAST : 0); s_hdr[1] = ip; }
         wide_bar_arrive(BAR_REC_FULL);
-        wide_bar_wait(BAR_REC_FREE);                       // warp E has the batch in registers (it answers at once)
+        WT_TIME(WT_P_REC_FREE, wide_bar_wait(BAR_REC_FREE));    // warp E has the batch in registers (it answers at once)
         k = 0;
     };
     for (int c = 0; c < nchunks; c++) {
         const int buf = c % NB;
         const int cp0 = CH * c - int(ph);
-        wide_bar_wait(BAR_FULL + buf);
+        WT_TIME(WT_P_FULL, wide_bar_wait(BAR_FULL + buf));
         const uint16_t* ds = dist_of(buf);
         const uint8_t* fls = flen_of(buf);
         const uint32_t* hm = hmask_of(buf);
@@ -373,7 +456,8 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
             while (m == 0 && ++w < uint32_t(MW)) m = hm[w];
             return m ? 32u * w + uint32_t(__ffs(int(m))) - 1u : uint32_t(CH);
         };
-        uint32_t q = search(uint32_t(max(ip - cp0, 0)));
+        uint32_t q;
+        WT_TIME(WT_P_SEARCH, q = search(uint32_t(max(ip - cp0, 0)))); WT_COUNT(WT_SEARCHES);
         uint32_t code = 0, dist = 0;
         if (q < uint32_t(CH)) { code = fls[q]; dist = ds[q]; }
         while (q < uint32_t(CH)) {
@@ -382,8 +466,8 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
             const uint32_t delta = code & 63u;
             uint32_t nq = q + delta;
             if (delta - 1u >= 62u) {                          // rare: the length is still open (63) or no hit among the next 32 positions (0)
-                if (delta) fl = 8u + uint32_t(extend(int(ms) + 8, int(dist), matchlimit - (int(ms) + 8)));
-                nq = search(q + fl);
+                if (delta) { WT_TIME(WT_P_EXTEND, fl = 8u + uint32_t(extend(int(ms) + 8, int(dist), matchlimit - (int(ms) + 8)))); WT_COUNT(WT_EXTENDS); }
+                WT_TIME(WT_P_SEARCH, nq = search(q + fl)); WT_COUNT(WT_SEARCHES);
             }
             // the next sequence's two loads go out before this one is booked: their latency is the chain's critical path
             // (unconditionally: nq is at most 62 entries past the chunk, still inside this CTA's shared memory, and a value
@@ -392,12 +476,14 @@ lz4_compress_wide_kernel(const uint8_t* __restrict__ src_base, const uint64_t* _
             if (lane == 0) s_rec[k] = make_uint2(ms | (dist << 16), fl);
             ip = int(ms + fl);
             q = nq; code = ncode; dist = ndist;
+            WT_COUNT(WT_SEQUENCES);
             if (++k == 32) flush(false);
         }
         if (c + NB < nchunks) wide_bar_arrive(BAR_FREE + buf);
     }
     flush(true);
     if (NW == 2) finish(ip);
+    WT_END(WT_P_TOTAL, WT_P_FULL, WT_N);
 }
 
 } // namespace b200

@@ -38,16 +38,21 @@ def main():
     ccap = torch.full((nblk,), bound, device=dev, dtype=torch.int32)
     comp = torch.zeros(nblk * stride, device=dev, dtype=torch.uint8)
     clen = torch.zeros(nblk, device=dev, dtype=torch.int32)
-    out = torch.zeros(nblk * bs, device=dev, dtype=torch.uint8)
-    res = torch.zeros(nblk, device=dev, dtype=torch.int32)
     B = L.batch
     N = nblk * bs
     t, med = timeit(lambda: B.compress_fast_batch_dev(src, soff, slen, comp, coff, ccap, clen, bs))
     C = int(clen.sum().item())
+    if os.environ.get("COMPRESS_ONLY"):      # no room for a decompress buffer at the bench's 524 288 blocks: digest the streams
+        h = torch.zeros(nblk, device=dev, dtype=torch.int64)
+        B.xxh64_batch_dev(comp, coff, clen, h, 0)
+        digest = int(h.sum().item()) & (2**64 - 1)
+        print(f"compress: {N/t/2**30:.1f} GiB/s best ({N/med/2**30:.1f} med)  ratio {N/C:.3f}  streams {digest:016x}", flush=True)
+        return
+    out = torch.zeros(nblk * bs, device=dev, dtype=torch.uint8)
+    res = torch.zeros(nblk, device=dev, dtype=torch.int32)
     out.zero_(); B.decompress_safe_batch_dev(comp, coff, clen, out, soff, slen, res)
     rt = bool((res == bs).all().item()) and bool(torch.equal(out, src))
     print(f"compress: {N/t/2**30:.1f} GiB/s best ({N/med/2**30:.1f} med)  ratio {N/C:.3f}  hbm {(N+C)/t/1e9:.0f} GB/s  roundtrip={rt}", flush=True)
-    if os.environ.get("COMPRESS_ONLY"): return
     t, med = timeit(lambda: B.decompress_safe_batch_dev(comp, coff, clen, out, soff, slen, res))
     ok = bool((res == bs).all().item()) and bool(torch.equal(out, src))
     print(f"decompress_safe: {N/t/2**30:.1f} GiB/s best ({N/med/2**30:.1f} med) ok={ok}  hbm {(N+C)/t/1e9:.0f} GB/s", flush=True)
