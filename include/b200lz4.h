@@ -227,6 +227,18 @@ void    b200lz4f_index_block_offsets(void* index, uint64_t* block_off);   /* b20
 int64_t b200lz4f_decode_dev(void* index, const uint8_t* d_src, uint8_t* d_slots, uint64_t* frame_off, uint64_t* frame_len,
                             int32_t* block_len_out, void* stream);
 void    b200lz4f_index_free(void* index);
+/* Device-resident LZ4 Frame writer (LZ4FrameOutputStream.java:178-251, as b200lz4f_compress_host_hc writes it) for nf
+ * independent frames.  Frame f is src_len[f] bytes at d_src + src_off[f] (src_off / src_len: HOST arrays of nf entries; the
+ * bytes are in device memory of the current device).  The frames are written back to back into d_dst (device, dst_capacity
+ * bytes), each one byte for byte the frame b200lz4f_compress_host_hc would write for the same bytes at the same 16-byte
+ * phase with the same bsCode / flags / hc_level; frame_off[f] / frame_len[f] (host, may be NULL) say where.  Ordered after
+ * the work already queued on `stream`; returns when the frames are in d_dst.
+ * Returns the total bytes written, or: -9 dst_capacity < sum of b200lz4f_compress_bound(src_len[f], bsCode);
+ * -10 content checksum requested for a frame longer than 0x7FFFFFFF bytes (the host writer's limit); B200LZ4_E_ARG, _CUDA,
+ * _NODEVICE.  Argument and size errors are found before anything is launched or written. */
+int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
+                              uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
+                              int bsCode, int flags, int hc_level, void* stream);
 
 /* ---------------------------------------------------------------- lz4-java's containers as whole-buffer calls
  * LZ4 Frame writer (LZ4FrameOutputStream.java:178-251): independent blocks of 64 KiB..4 MiB (bsCode 4..7), blocks that

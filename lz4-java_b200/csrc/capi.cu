@@ -26,14 +26,14 @@ static thread_local char tl_err[256] = "";
 static thread_local int tl_status = 0;          // B200LZ4_E_* of the last value-returning call (hashes, digests) on this thread
 static thread_local int tl_device = -1;          // -1: not chosen yet (defaults to device 0)
 
-static int fail_cuda(cudaError_t e, const char* where)
+int fail_cuda(cudaError_t e, const char* where)
 {
     snprintf(tl_err, sizeof tl_err, "%s: %s", where, cudaGetErrorString(e));
     if (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver || e == cudaErrorInitializationError)
         return tl_status = B200LZ4_E_NODEVICE;
     return tl_status = B200LZ4_E_CUDA;
 }
-static int fail_arg(const char* what) { snprintf(tl_err, sizeof tl_err, "invalid argument: %s", what); return tl_status = B200LZ4_E_ARG; }
+int fail_arg(const char* what) { snprintf(tl_err, sizeof tl_err, "invalid argument: %s", what); return tl_status = B200LZ4_E_ARG; }
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail_cuda(e_, #call); } while (0)
 
 static int ensure_device()
@@ -87,15 +87,15 @@ struct Slot {
 
 static constexpr int    NSLOTS = 3;
 static size_t chunk_span_init() { const char* e = getenv("B200LZ4_CHUNK_MB"); size_t mb = e ? (size_t)atol(e) : 256; if (mb < 1) mb = 1; return mb << 20; }
-static const size_t CHUNK_SPAN = chunk_span_init();    // bytes of src (and of dst) per pipeline chunk: >= 4096 64-KiB blocks,
+const size_t CHUNK_SPAN = chunk_span_init();           // bytes of src (and of dst) per pipeline chunk: >= 4096 64-KiB blocks,
                                                            // i.e. at least two full waves of warps on 132 SMs per launch
-static constexpr size_t CHUNK_BLOCKS = 1 << 16;
 
 struct Ctx {
     int device = -1;
     Slot slot[NSLOTS];
     // one-block path
     uint8_t* h_bounce = nullptr; size_t bounce_cap = 0;    // pinned: [src | dst]
+    FrameScratch frame;                                    // b200lz4f_compress_dev (containers.cu)
     ~Ctx() { /* process teardown frees device memory; explicit frees would race CUDA shutdown */ }
 };
 
@@ -177,9 +177,28 @@ struct PipelineGuard {
     ~PipelineGuard() { if (!completed) ctx_abandon(c); }
 };
 
+int get_frame_scratch(FrameScratch** out)
+{
+    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
+    FrameScratch& f = c->frame;
+    if (!f.st2) {
+        cudaError_t e = cudaStreamCreateWithFlags(&f.st2, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.fork, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.join, cudaEventDisableTiming);
+        if (e != cudaSuccess) {
+            if (f.st2) cudaStreamDestroy(f.st2);
+            if (f.fork) cudaEventDestroy(f.fork);
+            f.st2 = nullptr; f.fork = nullptr;
+            return fail_cuda(e, "creating the frame writer's checksum stream");
+        }
+    }
+    *out = &f;
+    return 0;
+}
+
 // Grow-or-keep staging: a buffer smaller than `need` bytes is replaced by one with need >> slack_shift more room plus
 // 4 KiB, so calls of about the same size keep their buffers.  Whatever still reads or writes the old buffer must be done.
-static int reserve_device(uint8_t*& p, size_t& cap, size_t need, int slack_shift = 2)
+int reserve_device(uint8_t*& p, size_t& cap, size_t need, int slack_shift)
 {
     if (need <= cap) return 0;
     if (p) CK(cudaFree(p));
@@ -188,7 +207,7 @@ static int reserve_device(uint8_t*& p, size_t& cap, size_t need, int slack_shift
     CK(cudaMalloc(&p, c)); cap = c;
     return 0;
 }
-static int reserve_pinned(uint8_t*& p, size_t& cap, size_t need)
+int reserve_pinned(uint8_t*& p, size_t& cap, size_t need)
 {
     if (need <= cap) return 0;
     if (p) CK(cudaFreeHost(p));

@@ -26,6 +26,13 @@
 #define B200_NANOSLEEP(ns) __nanosleep(ns)
 #endif
 
+// A kernel launch that the emulator build runs as well: <<<grid, block, 0, st>>> on the GPU, one CTA after the other there.
+#ifdef B200_HOST_SIM
+#define B200_LAUNCH(kernel, grid, block, st, ...) simt::launch((unsigned)(grid), (block), [&] { kernel(__VA_ARGS__); })
+#else
+#define B200_LAUNCH(kernel, grid, block, st, ...) kernel<<<(grid), (block), 0, (st)>>>(__VA_ARGS__)
+#endif
+
 namespace b200 {
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }

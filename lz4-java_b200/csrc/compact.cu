@@ -6,14 +6,17 @@
 
 namespace b200 {
 
-// exclusive scan of max(lens[i],0) over n <= ~10^5 entries by one CTA; writes out_off[] and *total
+// exclusive scan of max(lens[i],0) over n <= ~10^5 entries by one CTA; writes out_off[] and *total.  carry_in (a device
+// word, not `total`): where the scan starts, so a call cut into chunks carries its running offset from one chunk's scan to
+// the next without the host; NULL starts at 0.
 __global__ void __launch_bounds__(1024)
-compact_scan_kernel(const int32_t* __restrict__ lens, uint64_t* __restrict__ out_off, uint64_t* __restrict__ total, uint32_t n)
+compact_scan_kernel(const int32_t* __restrict__ lens, uint64_t* __restrict__ out_off, uint64_t* __restrict__ total, uint32_t n,
+                    const uint64_t* __restrict__ carry_in = nullptr)
 {
     __shared__ uint64_t warp_sum[32];
     __shared__ uint64_t carry;
     const int lane = lane_id(), warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
+    if (threadIdx.x == 0) carry = carry_in ? *carry_in : 0;
     __syncthreads();
     for (uint32_t base = 0; base < n; base += 1024) {
         const uint32_t i = base + threadIdx.x;
@@ -46,6 +49,13 @@ compact_gather_kernel(const uint8_t* __restrict__ slots, const uint64_t* __restr
     if (b >= n) return;
     const int len = lens[b];
     if (len > 0) warp_copy(out + out_off[b], slots + slot_off[b], len, lane_id());
+}
+
+// (the emulator build runs this one too: the device frame writer calls it)
+cudaError_t launch_scan(const int32_t* lens, uint64_t* out_off, uint64_t* total, const uint64_t* carry_in, size_t n, cudaStream_t st)
+{
+    B200_LAUNCH(compact_scan_kernel, 1, 1024, st, lens, out_off, total, (uint32_t)n, carry_in);
+    return cudaGetLastError();
 }
 
 #ifndef B200_HOST_SIM          // launchers: CUDA only

@@ -9,6 +9,9 @@
 // i.e. the CUDA kernels.  No hashing or codec arithmetic runs on the host.
 #include "../../include/b200lz4.h"
 #include "kernels.h"
+#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device frame writer's kernels come with it
+#include "frame_encode.cu"
+#endif
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -50,9 +53,7 @@ int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, si
     size_t o = 0;
     put32(dst, 0x184D2204u); o = 4;
     const size_t hdr = o;
-    dst[o++] = (uint8_t)((1 << 6) | (1 << 5) | ((flags & 2) ? 1 << 4 : 0) | ((flags & 4) ? 1 << 3 : 0) | ((flags & 1) ? 1 << 2 : 0));
-    dst[o++] = (uint8_t)(bsCode << 4);
-    if (flags & 4) { put32(dst + o, (uint32_t)n); put32(dst + o + 4, (uint32_t)((uint64_t)n >> 32)); o += 8; }
+    o += (size_t)b200::frame_descriptor(dst + o, bsCode, flags, n);
     const uint32_t hh = b200xxh32(dst + hdr, o - hdr, 0);                        // descriptor checksum (:187)
     if (hh == 0 && b200lz4_last_error()[0]) { /* a real zero hash is possible; device errors are caught below */ }
     dst[o++] = (uint8_t)((hh >> 8) & 0xFF);
@@ -90,6 +91,155 @@ int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, si
 }
 int64_t b200lz4f_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags)
 { return b200lz4f_compress_host_hc(src, n, dst, cap, bsCode, flags, 0); }
+
+} // extern "C"
+
+// ---------------------------------------------------------------- LZ4 Frame writer, device memory (frame_encode.cu)
+namespace b200 {
+
+// Where the FramePlan arrays of a call with nb blocks, ni items and nf frames lie in one blob, the same on the host and the
+// device.  f_off, f_end and the two carry words come last: one copy brings the results back.
+struct FramePlanLayout {
+    size_t b_soff, b_slen, b_slot, b_ccap, b_clen, b_poff, b_plen, b_sum;
+    size_t i_frame, i_block, i_size, i_off;
+    size_t f_soff, f_len, f_len32, f_sum, f_off, f_end, carry, bytes = 0;
+    FramePlanLayout(size_t nb, size_t ni, size_t nf)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        b_soff = take(8 * nb); b_slen = take(4 * nb); b_slot = take(8 * nb); b_ccap = take(4 * nb); b_clen = take(4 * nb);
+        b_poff = take(8 * nb); b_plen = take(4 * nb); b_sum = take(4 * nb);
+        i_frame = take(4 * ni); i_block = take(4 * ni); i_size = take(4 * ni); i_off = take(8 * ni);
+        f_soff = take(8 * nf); f_len = take(8 * nf); f_len32 = take(4 * nf); f_sum = take(4 * nf);
+        f_off = take(8 * nf); f_end = take(8 * nf); carry = take(16);
+    }
+};
+
+struct FrameChunk { size_t i0, i1, b0, b1; };                       // items [i0, i1), their blocks [b0, b1)
+
+static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
+                                   uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
+                                   int bsCode, int flags, int hc_level, cudaStream_t st)
+{
+    // ---- arguments and sizes: nothing is launched or written before these pass
+    if (bsCode < 4 || bsCode > 7) return fail_arg("bsCode must be 4..7");
+    if (nf == 0) return 0;
+    if (!src_off || !src_len || !d_dst) return fail_arg("null pointer");
+    const uint64_t bs = 1ull << (8 + 2 * bsCode);
+    uint64_t need = 0, nb = 0, ni = 0, bytes = 0;
+    bool too_long = false;
+    for (size_t f = 0; f < nf; f++) {
+        const uint64_t n = src_len[f];
+        if (n > (1ull << 47)) return fail_arg("src_len");
+        need += b200lz4f_compress_bound(n, bsCode);
+        nb += (n + bs - 1) / bs; ni += n ? (n + bs - 1) / bs : 1; bytes += n;
+        if ((flags & 1) && n > 0x7FFFFFFFull) too_long = true;
+    }
+    if (bytes && !d_src) return fail_arg("null pointer");
+    if (ni > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
+    if (need > dst_capacity) return -9;
+    if (too_long) return -10;                                       // the host writer's limit on a content checksum
+    FrameScratch* s; int rc = get_frame_scratch(&s); if (rc) return rc;
+    const FramePlanLayout L(nb, ni, nf);
+    rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
+    if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
+    if (rc) return rc;
+
+    // ---- plan: blocks of bs bytes (the last one of a frame short), items, and chunks of at most CHUNK_SPAN source bytes and
+    // CHUNK_BLOCKS items, so the compressed slots take the same room however large the call
+    uint8_t* H = s->h_plan;
+    auto h64 = [&](size_t o) { return (uint64_t*)(H + o); };
+    auto h32 = [&](size_t o) { return (int32_t*)(H + o); };
+    std::vector<FrameChunk> chunks;
+    size_t b = 0, i = 0, ci0 = 0, cb0 = 0;
+    uint64_t slot = 0, span = 0, slots_need = 0;
+    for (size_t f = 0; f < nf; f++) {
+        const uint64_t n = src_len[f], nbf = (n + bs - 1) / bs;
+        h64(L.f_soff)[f] = src_off[f]; h64(L.f_len)[f] = n; h32(L.f_len32)[f] = (int32_t)(n < 0x7FFFFFFFull ? n : 0x7FFFFFFFull);
+        for (uint64_t k = 0; k < (nbf ? nbf : 1); k++, i++) {
+            const uint64_t len = nbf ? (n - k * bs < bs ? n - k * bs : bs) : 0;
+            if (i > ci0 && (i - ci0 >= CHUNK_BLOCKS || span + len > CHUNK_SPAN)) {
+                chunks.push_back(FrameChunk{ ci0, i, cb0, b });
+                slots_need = slot > slots_need ? slot : slots_need;
+                ci0 = i; cb0 = b; slot = 0; span = 0;
+            }
+            h32(L.i_frame)[i] = (int32_t)f;
+            h32(L.i_block)[i] = nbf ? (int32_t)b : -1;
+            if (!nbf) continue;
+            h64(L.b_soff)[b] = src_off[f] + k * bs; h32(L.b_slen)[b] = (int32_t)len;
+            h64(L.b_slot)[b] = slot; h32(L.b_ccap)[b] = (int32_t)compress_bound(len);
+            slot += aligned_compress_bound(len); span += len; b++;
+        }
+    }
+    chunks.push_back(FrameChunk{ ci0, i, cb0, b });
+    slots_need = slot > slots_need ? slot : slots_need;
+    h64(L.carry)[0] = 0;
+    rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
+
+    uint8_t* D = s->d_plan;
+    const FramePlan P{ d_src, d_dst, s->d_slots,
+                       (const uint64_t*)(D + L.b_soff), (const int32_t*)(D + L.b_slen), (const uint64_t*)(D + L.b_slot), (const int32_t*)(D + L.b_clen),
+                       (uint64_t*)(D + L.b_poff), (int32_t*)(D + L.b_plen), (const uint32_t*)(D + L.b_sum),
+                       (const uint32_t*)(D + L.i_frame), (const int32_t*)(D + L.i_block), (int32_t*)(D + L.i_size), (uint64_t*)(D + L.i_off),
+                       (const uint64_t*)(D + L.f_len), (const uint32_t*)(D + L.f_sum), (uint64_t*)(D + L.f_off), (uint64_t*)(D + L.f_end),
+                       (uint32_t)ni, bsCode, flags };
+    uint64_t* carry = (uint64_t*)(D + L.carry);
+
+    // ---- launches, all ordered after what `st` already holds.  A failure waits for what was queued: the scratch stays
+    // the thread's, and the next call may reuse or free it.
+    struct Drain {
+        cudaStream_t a, b; bool done = false;
+        ~Drain() { if (!done) { cudaStreamSynchronize(a); cudaStreamSynchronize(b); } }
+    } drain{ st, s->st2 };
+#define FCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail_cuda(e_, #call); } while (0)
+    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+    FCK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
+    if (flags & 1) {                // content checksums: the sources only, so from the start, beside everything else
+        FCK(cudaEventRecord(s->fork, st));
+        FCK(cudaStreamWaitEvent(s->st2, s->fork, 0));
+        FCK(counted(launch_xxh32_long(d_src, (const uint64_t*)(D + L.f_soff), (const int32_t*)(D + L.f_len32), 0,
+                                      (uint32_t*)(D + L.f_sum), nf, s->st2)));
+        FCK(cudaEventRecord(s->join, s->st2));
+    }
+    for (size_t k = 0; k < chunks.size(); k++) {
+        const FrameChunk& c = chunks[k];
+        if (c.b1 > c.b0) {          // the host writer's compressor and dispatch (compress_blocks above)
+            const BatchArgs a{ d_src, P.b_soff + c.b0, P.b_slen + c.b0, s->d_slots, P.b_slot + c.b0,
+                               (const int32_t*)(D + L.b_ccap) + c.b0, (int32_t*)P.b_clen + c.b0, c.b1 - c.b0 };
+            FCK(counted(hc_level > 0 ? launch_compress_hc(a, hc_level, st) : launch_compress_fast(a, bs <= 65536 ? 65536 : 0, st)));
+        }
+        const uint32_t i0 = (uint32_t)c.i0, n = (uint32_t)(c.i1 - c.i0);
+        FCK(counted(launch_frame_sizes(P, i0, n, st)));
+        FCK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
+        FCK(counted(launch_frame_emit(P, i0, n, st)));
+    }
+    if ((flags & 2) && nb) {        // block checksums over the payloads as written; the source average bounds the payloads'
+        FCK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+            d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
+    }
+    if (flags & 1) FCK(cudaStreamWaitEvent(st, s->join, 0));
+    FCK(counted(launch_frame_seal(P, st)));
+    FCK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
+    FCK(cudaStreamSynchronize(st));
+#undef FCK
+    drain.done = true;
+    for (size_t f = 0; f < nf; f++) {
+        if (frame_off) frame_off[f] = h64(L.f_off)[f];
+        if (frame_len) frame_len[f] = h64(L.f_end)[f] - h64(L.f_off)[f];
+    }
+    return (int64_t)h64(L.carry)[chunks.size() & 1];
+}
+
+} // namespace b200
+
+extern "C" {
+
+int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
+                              uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
+                              int bsCode, int flags, int hc_level, void* stream)
+{
+    return b200::compress_frames_dev(d_src, src_off, src_len, nf, d_dst, dst_capacity, frame_off, frame_len, bsCode, flags,
+                                     hc_level, (cudaStream_t)stream);
+}
 
 // ---------------------------------------------------------------- "LZ4Block" container
 static const uint8_t LZ4BLOCK_MAGIC[8] = { 'L', 'Z', '4', 'B', 'l', 'o', 'c', 'k' };

@@ -77,6 +77,41 @@ def compress_frame(src, block_size_code: int = 4, content_checksum=True, block_c
     return out[:r].tobytes()
 
 
+def compress_frames_dev(src, src_off, src_len, block_size_code: int = 4, content_checksum=True, block_checksum=False,
+                        content_size=False, hc_level: int = 0, out=None):
+    """independent LZ4 frames of bytes already in device memory, written on the device (b200lz4f_compress_dev): frame f is
+    src[src_off[f] : src_off[f] + src_len[f]], byte for byte what compress_frame writes for the same bytes at the same 16-byte
+    phase.  src: a uint8 CUDA tensor; src_off / src_len: host sequences; out: a uint8 CUDA tensor on src's device (default: a
+    new one of the summed frame bounds).  Runs on torch's current stream and returns when the frames are written.
+    -> (out[:total], frame_off, frame_len), the last two np.uint64 arrays (where each frame lies in out)"""
+    import torch
+    off = np.ascontiguousarray(np.asarray(src_off, dtype=np.uint64).reshape(-1))
+    ln = np.ascontiguousarray(np.asarray(src_len, dtype=np.uint64).reshape(-1))
+    if len(off) != len(ln):
+        raise ValueError("src_off and src_len must have the same length")
+    if src.dtype != torch.uint8 or not src.is_cuda or not src.is_contiguous():
+        raise ValueError("src must be a contiguous uint8 CUDA tensor")
+    if len(ln) and int((off + ln).max()) > src.numel():
+        raise ValueError("a frame reaches past the end of src")
+    if not 4 <= block_size_code <= 7:
+        raise ValueError("block_size_code must be 4..7 (64 KiB .. 4 MiB)")
+    L = N.lib()
+    bounds = [L.b200lz4f_compress_bound(int(n), block_size_code) for n in ln]
+    if out is None:
+        out = torch.empty(max(sum(bounds), 1), dtype=torch.uint8, device=src.device)
+    elif out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    flags = (1 if content_checksum else 0) | (2 if block_checksum else 0) | (4 if content_size else 0)
+    frame_off, frame_len = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
+    r = L.b200lz4f_compress_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(), out.numel(),
+                                frame_off.ctypes.data, frame_len.ctypes.data, block_size_code, flags, hc_level,
+                                torch.cuda.current_stream(src.device).cuda_stream)
+    N.check(r)
+    if r < 0:
+        raise LZ4FrameError(int(r))
+    return out[:r], frame_off, frame_len
+
+
 # ---- lz4-java's private "LZ4Block" container (LZ4BlockOutputStream / LZ4BlockInputStream)
 def compress_lz4block(src, block_size: int = 1 << 16, hc_level: int = 0) -> bytes:
     s = _view(src)
