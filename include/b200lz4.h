@@ -227,6 +227,26 @@ void    b200lz4f_index_block_offsets(void* index, uint64_t* block_off);   /* b20
 int64_t b200lz4f_decode_dev(void* index, const uint8_t* d_src, uint8_t* d_slots, uint64_t* frame_off, uint64_t* frame_len,
                             int32_t* block_len_out, void* stream);
 void    b200lz4f_index_free(void* index);
+/* The index of a container in DEVICE memory: d_src holds srcSize bytes in memory of the current device.  The same index
+ * b200lz4f_index_create (single == 0) or _single (single != 0) builds from the same bytes -- same *err, *slot_bytes,
+ * *src_consumed, blocks, block offsets and stream-order verdict -- and the calls above take it unchanged.  The container is
+ * walked on the device; only per-frame and per-block facts come to the host, no payload byte.  Ordered after the work already
+ * queued on `stream`; returns when the index is built.
+ * frame_hint (HOST array of nhint offsets, may be NULL): where the caller believes frames start (b200lz4f_compress_dev's
+ * frame_off).  The stretches between hints are walked in parallel, one device thread each; one frame is always walked by one
+ * thread, so a single frame of many small blocks is a serial chain of dependent loads whatever the hints.  Hints need not be
+ * right: any hints give the index of no hints, a wrong one only costs time.  They must be ascending and below srcSize, or
+ * the call returns NULL with *err = B200LZ4_E_ARG before anything is launched. */
+void*   b200lz4f_index_create_dev(const uint8_t* d_src, size_t srcSize, int single, const uint64_t* frame_hint, size_t nhint,
+                                  uint64_t* slot_bytes, size_t* src_consumed, int* err, void* stream);
+/* b200lz4f_decompress_host / _single with d_src and d_dst in device memory of the current device (hints as above): the same
+ * total or code (-1 .. -10; -9 when dstCapacity is too small), the same content packed into d_dst[0, total).  On an error
+ * d_dst is not written at all, on success nothing past total.  Besides d_dst the call needs slot_bytes of device scratch
+ * (see b200lz4f_index_create_dev; about the content size rounded up to whole blocks), kept by the calling thread for its next
+ * calls; a caller short of memory calls b200lz4f_index_create_dev and b200lz4f_decode_dev into a buffer of its own.
+ * Ordered after the work already queued on `stream`; returns when d_dst holds the content. */
+int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t srcSize, uint8_t* d_dst, size_t dstCapacity, int single,
+                                const uint64_t* frame_hint, size_t nhint, size_t* src_consumed, void* stream);
 /* Device-resident LZ4 Frame writer (LZ4FrameOutputStream.java:178-251, as b200lz4f_compress_host_hc writes it) for nf
  * independent frames.  Frame f is src_len[f] bytes at d_src + src_off[f] (src_off / src_len: HOST arrays of nf entries; the
  * bytes are in device memory of the current device).  The frames are written back to back into d_dst (device, dst_capacity

@@ -96,6 +96,7 @@ struct Ctx {
     // one-block path
     uint8_t* h_bounce = nullptr; size_t bounce_cap = 0;    // pinned: [src | dst]
     FrameScratch frame;                                    // b200lz4f_compress_dev (containers.cu)
+    FrameReadScratch frame_read;                           // b200lz4f_index_create_dev / b200lz4f_decompress_dev (frame.cu)
     ~Ctx() { /* process teardown frees device memory; explicit frees would race CUDA shutdown */ }
 };
 
@@ -193,6 +194,13 @@ int get_frame_scratch(FrameScratch** out)
         }
     }
     *out = &f;
+    return 0;
+}
+
+int get_frame_read_scratch(FrameReadScratch** out)
+{
+    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
+    *out = &c->frame_read;
     return 0;
 }
 

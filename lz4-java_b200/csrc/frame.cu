@@ -13,8 +13,14 @@
 //      beside the decoder on a second stream, taking each block as soon as it is decoded
 // Blocks of one frame are decoded in parallel because lz4-java only writes independent blocks
 // (LZ4FrameOutputStream.java:58,361-363; dependent blocks are rejected like the reference does).
+// With the container in device memory (b200lz4f_index_create_dev, b200lz4f_decompress_dev) the index pass itself runs on the
+// device (frame_index.cu) and only its records come to the host; both indexers run the same walk (walk_frames, kernels.h).
 #include "../../include/b200lz4.h"
 #include "kernels.h"
+#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device indexer's kernels come with it
+#include "frame_index.cu"
+#endif
+#include <algorithm>
 #include <cstring>
 #include <new>
 #include <vector>
@@ -23,8 +29,6 @@ namespace b200 {
 
 cudaError_t launch_gather(const uint8_t* src, const uint64_t* src_off, const int32_t* lens,
                           uint8_t* dst, const uint64_t* dst_off, size_t n, cudaStream_t st);
-
-static inline uint32_t rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
 
 struct FrameRec {
     uint64_t desc_off; int32_t desc_len; uint8_t hc_byte; uint8_t flg; uint32_t bs;
@@ -58,78 +62,201 @@ struct FrameIndex {
     std::vector<size_t> comp_ix, raw_ix, bsum_ix, fsum_ix;
 };
 
-// LZ4FrameInputStream.nextFrameInfo / readHeader / readBlock as a pure index pass.  The reader is a stream: it hands out the
-// bytes of every frame before a malformed spot and fails THERE, after any checksum or decode error that lies earlier.  So an
-// error behind at least one indexed frame is not returned here: it is kept in ix.tail_err, what precedes it is decoded and
-// verified like any other input (the blocks of a frame cut short included -- that frame has no content checks), and
-// decode_dev reports the first error in stream order.
-static int index_frames(const uint8_t* src, size_t n, FrameIndex& ix, bool single = false, size_t* consumed = nullptr)
-{
-    size_t ip = 0; bool seen = false;
-    int err = 0;
-    FrameRec f{};
-    auto stop = [&](int code) { err = code; };
-    while (ip < n && !err) {
-        if (n - ip < 4) { stop(-1); break; }
-        const uint32_t magic = rd32(src + ip); ip += 4;
-        if ((magic >> 4) == (0x184D2A50u >> 4)) {                               // skippable (:154,162-173)
-            if (n - ip < 4) { stop(-1); break; }
-            const uint32_t sz = rd32(src + ip); ip += 4;
-            if (n - ip < sz) { stop(-1); break; }
-            ip += sz; seen = true; continue;
-        }
-        if (magic != 0x184D2204u) { stop(-2); break; }                          // (:151)
+// The host sink of walk_frames (kernels.h): frames and blocks into the index, each block with its slot.  The device indexer
+// replays its walkers' records through it, so both indexers lay out slots the same way.
+struct IndexSink {
+    FrameIndex& ix; FrameRec f{};
+    void frame_begin(const WalkFrame& w)
+    {
         f = FrameRec{};
-        f.desc_off = ip;
-        if (n - ip < 3) { stop(-1); break; }
-        f.flg = src[ip++]; const uint8_t bd = src[ip++];
-        if ((f.flg >> 6) != 1 || (f.flg & 2) || !(f.flg & 0x20) || (f.flg & 1)) { stop(-10); break; }   // version, reserved, B.Indep, dictID
-        if ((bd & 0x8F) || (bd >> 4) < 4) { stop(-10); break; }
-        f.bs = 1u << (8 + 2 * (bd >> 4));
-        f.has_size = f.flg & 8;
-        if (f.has_size) { if (n - ip < 9) { stop(-1); break; } f.content_size = (uint64_t)rd32(src + ip) | ((uint64_t)rd32(src + ip + 4) << 32); ip += 8; }
-        if (n - ip < 1) { stop(-1); break; }
-        f.desc_len = (int32_t)(ip - f.desc_off);
-        f.hc_byte = src[ip++];
+        f.desc_off = w.desc_off; f.desc_len = w.desc_len; f.hc_byte = w.hc_byte; f.flg = w.flg;
+        f.bs = 1u << (8 + 2 * (w.bd >> 4));
         f.first_block = ix.blocks.size();
         f.out_off = ix.slot_bytes;
-        for (;;) {                                                              // readBlock (:258-321)
-            if (n - ip < 4) { stop(-1); break; }
-            const uint32_t word = rd32(src + ip); ip += 4;
-            const uint32_t sz = word & 0x7FFFFFFFu;
-            if (sz == 0) break;                                                 // EndMark
-            if (sz > f.bs) { stop(-4); break; }
-            BlockRec b{}; b.src_off = ip; b.size = sz; b.raw = word >> 31; b.frame = ix.frames.size();
-            if (n - ip < sz) { stop(-1); break; }
-            ip += sz;
-            b.has_checksum = f.flg & 0x10;
-            if (b.has_checksum) { if (n - ip < 4) { stop(-1); break; } b.checksum = rd32(src + ip); ip += 4; }
-            // the slot: a stored block needs its own size, a compressed one cannot decode to more than 255 bytes per byte
-            // (one length byte adds at most 255) -- so a stream of tiny flushed blocks asks for what it can fill, not for
-            // blockMaxSize each.  Full blocks keep exactly bs: a frame without short blocks in the middle stays contiguous.
-            const uint64_t room = b.raw ? sz : std::min<uint64_t>(f.bs, 255ull * sz);
-            b.cap = (uint32_t)room;
-            b.out_off = ix.slot_bytes; ix.slot_bytes += room >= f.bs ? f.bs : ((room + 15) & ~15ull);
-            ix.blocks.push_back(b);
-        }
-        f.nblocks = ix.blocks.size() - f.first_block;
-        f.complete = !err;
-        f.has_checksum = !err && (f.flg & 4);
-        if (f.has_checksum) {
-            if (n - ip < 4) { stop(-1); f.complete = false; f.has_checksum = false; }
-            else { f.content_checksum = rd32(src + ip); ip += 4; }
-        }
-        if (!f.complete) f.has_size = false;
-        ix.frames.push_back(f); seen = true;
-        if (single) break;                                                      // readSingleFrame (:83-91, 327, 346): the rest is not read
     }
-    if (consumed) *consumed = ip;
+    void block(uint64_t src_off, uint32_t word, uint32_t checksum)
+    {
+        BlockRec b{}; b.src_off = src_off; b.size = word & 0x7FFFFFFFu; b.raw = word >> 31; b.frame = ix.frames.size();
+        b.has_checksum = f.flg & 0x10;
+        if (b.has_checksum) b.checksum = checksum;
+        // the slot: a stored block needs its own size, a compressed one cannot decode to more than 255 bytes per byte
+        // (one length byte adds at most 255) -- so a stream of tiny flushed blocks asks for what it can fill, not for
+        // blockMaxSize each.  Full blocks keep exactly bs: a frame without short blocks in the middle stays contiguous.
+        const uint64_t room = b.raw ? b.size : std::min<uint64_t>(f.bs, 255ull * b.size);
+        b.cap = (uint32_t)room;
+        b.out_off = ix.slot_bytes; ix.slot_bytes += room >= f.bs ? f.bs : ((room + 15) & ~15ull);
+        ix.blocks.push_back(b);
+    }
+    void frame_end(const WalkFrame& w)
+    {
+        f.nblocks = ix.blocks.size() - f.first_block;
+        f.content_size = w.content_size; f.has_size = w.has_size;
+        f.content_checksum = w.content_checksum; f.has_checksum = w.has_checksum;
+        f.complete = w.complete;
+        ix.frames.push_back(f);
+    }
+};
+
+// What the whole container's walk means for the index.  The reader is a stream: it hands out the bytes of every frame before
+// a malformed spot and fails THERE, after any checksum or decode error that lies earlier.  So an error behind at least one
+// indexed frame is not returned here: it is kept in ix.tail_err, what precedes it is decoded and verified like any other
+// input (the blocks of a frame cut short included -- that frame has no content checks), and decode_dev reports the first
+// error in stream order.
+static int index_verdict(FrameIndex& ix, int err, bool seen)
+{
     if (err) {
         if (ix.frames.empty()) return err;                                      // nothing lies before the error
         ix.tail_err = err;
         return 0;
     }
     return seen ? 0 : -1;
+}
+
+// LZ4FrameInputStream.nextFrameInfo / readHeader / readBlock as a pure index pass over host memory
+static int index_frames(const uint8_t* src, size_t n, FrameIndex& ix, bool single = false, size_t* consumed = nullptr)
+{
+    IndexSink sink{ ix };
+    const WalkEnd e = walk_frames(src, n, 0, n, single, sink);
+    if (consumed) *consumed = e.ip;
+    return index_verdict(ix, e.err, e.seen);
+}
+
+// ---- the same index from bytes in device memory (walkers: frame_index.cu).  Only records come back, never payload.
+// Where the arrays of one walk with m walkers lie, the same in d_seg and h_seg: the segments go up, the rest comes back.
+struct WalkLayout {
+    size_t segs, sums, lens, pos, total, bytes = 0;
+    explicit WalkLayout(size_t m)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        segs = take(sizeof(WalkSeg) * m); sums = take(sizeof(WalkSummary) * m); lens = take(4 * m); pos = take(8 * m); total = take(16);
+    }
+};
+static constexpr uint64_t WALK_MAX_REC = 0x7FFFFFFFull;      // records of one walker (the packing scan counts in int32)
+
+// One walker per segment: summaries into sum[], the records each walker wrote appended to recs (walker j's from rec_at[j]).
+// A region guess that proved too small is run once more, for those walkers only, with room for exactly what they counted.
+static int walk_segments(FrameReadScratch& s, const uint8_t* d_src, uint64_t n, bool single, const uint64_t* start, const uint64_t* end,
+                         size_t m, WalkSummary* sum, uint64_t* rec_at, std::vector<WalkRec>& recs, cudaStream_t st)
+{
+    std::vector<size_t> todo(m);
+    std::vector<uint64_t> cap(m);
+    for (size_t j = 0; j < m; j++) { todo[j] = j; cap[j] = std::min(((end[j] - start[j]) >> 12) + 64, WALK_MAX_REC); }   // ~ one per 4 KiB
+#define WCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail_cuda(e_, #call); } while (0)
+    while (!todo.empty()) {
+        const size_t k = todo.size();
+        const WalkLayout L(k);
+        uint64_t room = 0;
+        for (size_t i = 0; i < k; i++) room += cap[todo[i]];
+        int rc = reserve_device(s.d_seg, s.seg_cap, L.bytes);
+        if (!rc) rc = reserve_pinned(s.h_seg, s.h_seg_cap, std::max<size_t>(L.bytes, room * sizeof(WalkRec)));
+        if (!rc) rc = reserve_device(s.d_recs, s.recs_cap, room * sizeof(WalkRec) + 16);
+        if (!rc) rc = reserve_device(s.d_packed, s.packed_cap, room * sizeof(WalkRec) + 16);
+        if (rc) return rc;
+        WalkSeg* hs = (WalkSeg*)(s.h_seg + L.segs);
+        uint64_t at = 0;
+        for (size_t i = 0; i < k; i++) { const size_t j = todo[i]; hs[i] = WalkSeg{ start[j], end[j], at, cap[j] }; at += cap[j]; }
+        uint8_t* D = s.d_seg;
+        WCK(cudaMemcpyAsync(D, s.h_seg, L.sums, cudaMemcpyHostToDevice, st));
+        g_launch_count.fetch_add(3, std::memory_order_relaxed);
+        WCK(launch_frame_walk(d_src, n, single, (const WalkSeg*)D, (WalkSummary*)(D + L.sums), (int32_t*)(D + L.lens), (WalkRec*)s.d_recs, (uint32_t)k, st));
+        WCK(launch_scan((const int32_t*)(D + L.lens), (uint64_t*)(D + L.pos), (uint64_t*)(D + L.total), nullptr, k, st));
+        WCK(launch_frame_pack((const WalkSeg*)D, (const int32_t*)(D + L.lens), (const uint64_t*)(D + L.pos), (const WalkRec*)s.d_recs,
+                              (WalkRec*)s.d_packed, (uint32_t)k, st));
+        WCK(cudaMemcpyAsync(s.h_seg + L.sums, D + L.sums, L.bytes - L.sums, cudaMemcpyDeviceToHost, st));
+        WCK(cudaStreamSynchronize(st));
+        const uint64_t packed = *(const uint64_t*)(s.h_seg + L.total);
+        const WalkSummary* hsum = (const WalkSummary*)(s.h_seg + L.sums);
+        const uint64_t* hpos = (const uint64_t*)(s.h_seg + L.pos);
+        std::vector<WalkSummary> got(hsum, hsum + k);
+        std::vector<uint64_t> pos(hpos, hpos + k);
+        if (packed) {
+            WCK(cudaMemcpyAsync(s.h_seg, s.d_packed, packed * sizeof(WalkRec), cudaMemcpyDeviceToHost, st));
+            WCK(cudaStreamSynchronize(st));
+        }
+        const size_t base = recs.size();
+        recs.insert(recs.end(), (const WalkRec*)s.h_seg, (const WalkRec*)s.h_seg + packed);
+        std::vector<size_t> again;
+        for (size_t i = 0; i < k; i++) {
+            const size_t j = todo[i];
+            sum[j] = got[i]; rec_at[j] = base + pos[i];
+            if (got[i].nrec > cap[j]) {
+                if (got[i].nrec > WALK_MAX_REC) return fail_arg("more than 2^31 frames and blocks between two frame hints");
+                cap[j] = got[i].nrec; again.push_back(j);
+            }
+        }
+        todo.swap(again);
+    }
+#undef WCK
+    return 0;
+}
+
+// walker records -> the index, through the host indexer's own sink (records: frame_index.cu, RecordSink)
+static void replay(const WalkRec* r, uint64_t nrec, IndexSink& sink)
+{
+    for (uint64_t i = 0; i + 2 <= nrec;) {
+        WalkFrame f{};
+        const uint32_t bits = (uint32_t)(r[i + 1].b >> 32);
+        f.desc_off = r[i].a; f.content_size = r[i].b; f.nblocks = r[i + 1].a; f.content_checksum = (uint32_t)r[i + 1].b;
+        f.flg = (uint8_t)bits; f.bd = (uint8_t)(bits >> 8); f.hc_byte = (uint8_t)(bits >> 16); f.desc_len = (uint8_t)((bits >> 24) & 15);
+        f.complete = bits & (1u << 28); f.has_checksum = bits & (1u << 29); f.has_size = bits & (1u << 30);
+        i += 2;
+        sink.frame_begin(f);
+        for (uint64_t k = 0; k < f.nblocks; k++, i++) sink.block(r[i].a, (uint32_t)r[i].b, (uint32_t)(r[i].b >> 32));
+        sink.frame_end(f);
+    }
+}
+
+// The chain of the container from offset 0, stitched from walkers that started at the hints.  Where it does not land on a
+// hint, a walker is run from where it is to the next hint: a wrong hint costs a launch, never a different index.
+static int index_frames_dev(FrameReadScratch& s, const uint8_t* d_src, uint64_t n, bool single, const uint64_t* hint, size_t nhint,
+                            FrameIndex& ix, size_t* consumed, cudaStream_t st)
+{
+    const size_t m = nhint + 1;
+    std::vector<uint64_t> start(m), end(m), rec_at(m);
+    start[0] = 0;
+    for (size_t j = 0; j < nhint; j++) { end[j] = hint[j]; start[j + 1] = hint[j]; }
+    end[nhint] = n;
+    std::vector<WalkSummary> sum(m);
+    std::vector<WalkRec> recs;
+    int rc = walk_segments(s, d_src, n, single, start.data(), end.data(), m, sum.data(), rec_at.data(), recs, st);
+    if (rc) return rc;
+    IndexSink sink{ ix };
+    WalkSummary cur = sum[0]; uint64_t cur_at = rec_at[0];
+    size_t next = 1;
+    bool seen = false;
+    for (;;) {
+        replay(recs.data() + cur_at, cur.nrec, sink);
+        seen |= cur.flags & WALK_SEEN;
+        if (cur.err || (cur.flags & WALK_SINGLE_DONE) || cur.ip >= n) break;
+        while (next < m && start[next] < cur.ip) next++;
+        if (next < m && start[next] == cur.ip) { cur = sum[next]; cur_at = rec_at[next]; next++; continue; }
+        const uint64_t from = cur.ip, to = next < m ? start[next] : n;
+        rc = walk_segments(s, d_src, n, single, &from, &to, 1, &cur, &cur_at, recs, st);
+        if (rc) return rc;
+    }
+    if (consumed) *consumed = cur.ip;
+    return index_verdict(ix, cur.err, seen);
+}
+
+// Packs decoded blocks back to back: block b's blen[b] bytes move from d_slots + its slot to d_dst + the lengths before it.
+// d_desc: device room for pack_desc_bytes(blocks) of descriptors.  One launch; ordered on st.
+static size_t pack_desc_bytes(size_t nb) { return 2 * ((nb * 8 + 15) & ~size_t(15)) + nb * 4; }
+static cudaError_t pack_blocks(const FrameIndex& ix, const int32_t* blen, const uint8_t* d_slots, uint8_t* d_dst, uint8_t* d_desc, cudaStream_t st)
+{
+    const size_t nb = ix.blocks.size();
+    if (nb == 0) return cudaSuccess;
+    const size_t o_to = (nb * 8 + 15) & ~size_t(15), o_len = 2 * o_to;
+    std::vector<uint8_t> h(pack_desc_bytes(nb));
+    uint64_t pos = 0;
+    for (size_t b = 0; b < nb; b++) {
+        ((uint64_t*)h.data())[b] = ix.blocks[b].out_off;
+        ((uint64_t*)(h.data() + o_to))[b] = pos; pos += (uint64_t)blen[b];
+    }
+    memcpy(h.data() + o_len, blen, nb * 4);
+    const cudaError_t e = cudaMemcpyAsync(d_desc, h.data(), h.size(), cudaMemcpyHostToDevice, st);   // pageable: staged before it returns
+    if (e != cudaSuccess) return e;
+    g_launch_count += 1;
+    return launch_gather(d_slots, (const uint64_t*)d_desc, (const int32_t*)(d_desc + o_len), d_dst, (const uint64_t*)(d_desc + o_to), nb, st);
 }
 
 template <typename T> static size_t put(std::vector<uint8_t>& blob, size_t count)
@@ -206,6 +333,30 @@ void* b200lz4f_index_create(const uint8_t* src_host, size_t n, uint64_t* slot_by
 { return index_create(src_host, n, false, slot_bytes, nullptr, err); }
 void* b200lz4f_index_create_single(const uint8_t* src_host, size_t n, uint64_t* slot_bytes, size_t* src_consumed, int* err)
 { return index_create(src_host, n, true, slot_bytes, src_consumed, err); }
+
+void* b200lz4f_index_create_dev(const uint8_t* d_src, size_t n, int single, const uint64_t* frame_hint, size_t nhint,
+                                uint64_t* slot_bytes, size_t* src_consumed, int* err, void* stream)
+{
+    auto fail = [&](int rc) -> void* { if (err) *err = rc; return nullptr; };
+    if (nhint && !frame_hint) return fail(fail_arg("frame_hint is NULL"));
+    for (size_t j = 0; j < nhint; j++)
+        if (frame_hint[j] >= n || (j && frame_hint[j] < frame_hint[j - 1])) return fail(fail_arg("frame hints must be ascending and below srcSize"));
+    if (n && !d_src) return fail(fail_arg("null pointer"));
+    if (n == 0) { if (src_consumed) *src_consumed = 0; return fail(-1); }      // no frame at all, like index_create
+    FrameReadScratch* s;
+    int rc = get_frame_read_scratch(&s);
+    if (rc) return fail(rc);
+    FrameIndex* ix = new (std::nothrow) FrameIndex();
+    if (!ix) return fail(fail_arg("out of host memory"));
+    const cudaStream_t st = (cudaStream_t)stream;
+    rc = index_frames_dev(*s, d_src, n, single != 0, frame_hint, nhint, *ix, src_consumed, st);
+    if (rc == B200LZ4_E_CUDA) cudaStreamSynchronize(st);                        // a failed call leaves nothing running on the scratch
+    if (rc == 0) rc = build_descriptors(*ix);
+    if (rc) { delete ix; return fail(rc); }
+    if (slot_bytes) *slot_bytes = ix->slot_bytes;
+    if (err) *err = 0;
+    return ix;
+}
 
 // getExpectedContentSize / isExpectedContentSizeDefined (:416-445): the content size the first non-skippable frame declares,
 // -1 when it declares none or when there is no frame at all; the descriptor hash is verified like nextFrameInfo does.
@@ -385,20 +536,14 @@ static int64_t decompress_host(const uint8_t* src, size_t n, uint8_t* dst, size_
         } else {
             // short blocks in mid-frame (everything is verified already): the device packs the blocks, one copy brings them back
             rc = 0;
-            const size_t nb = ix.blocks.size();
-            std::vector<uint64_t> from(nb), to(nb);
-            for (size_t b = 0; b < nb; b++) { from[b] = ix.blocks[b].out_off; to[b] = pos; pos += (uint64_t)blen[b]; }
+            for (size_t b = 0; b < ix.blocks.size(); b++) pos += (uint64_t)blen[b];
             if (pos > dst_capacity) { rc = -9; ok = false; }
             uint8_t* d_tmp = nullptr;
-            const size_t o_to = (nb * 8 + 15) & ~size_t(15), o_len = 2 * o_to, o_out = (o_len + nb * 4 + 15) & ~size_t(15);
+            const size_t o_out = (pack_desc_bytes(ix.blocks.size()) + 15) & ~size_t(15);
             if (ok && pos) {
                 if (cudaMalloc(&d_tmp, o_out + pos + 16) != cudaSuccess) { rc = B200LZ4_E_CUDA; ok = false; d_tmp = nullptr; }
-                if (ok && (cudaMemcpyAsync(d_tmp, from.data(), nb * 8, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-                           cudaMemcpyAsync(d_tmp + o_to, to.data(), nb * 8, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-                           cudaMemcpyAsync(d_tmp + o_len, blen.data(), nb * 4, cudaMemcpyHostToDevice, st) != cudaSuccess)) { rc = B200LZ4_E_CUDA; ok = false; }
                 if (ok) {
-                    g_launch_count += 1;
-                    if (launch_gather(d_slots, (uint64_t*)d_tmp, (int32_t*)(d_tmp + o_len), d_tmp + o_out, (uint64_t*)(d_tmp + o_to), nb, st) != cudaSuccess ||
+                    if (pack_blocks(ix, blen.data(), d_slots, d_tmp + o_out, d_tmp, st) != cudaSuccess ||
                         cudaMemcpyAsync(dst, d_tmp + o_out, pos, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
                         cudaStreamSynchronize(st) != cudaSuccess) { rc = B200LZ4_E_CUDA; ok = false; }
                 }
@@ -419,5 +564,36 @@ int64_t b200lz4f_decompress_host(const uint8_t* src, size_t n, uint8_t* dst, siz
 // LZ4FrameInputStream(in, readSingleFrame = true): the first non-skippable frame only; *src_consumed = where it ended
 int64_t b200lz4f_decompress_host_single(const uint8_t* src, size_t n, uint8_t* dst, size_t dst_capacity, size_t* src_consumed)
 { return decompress_host(src, n, dst, dst_capacity, true, src_consumed); }
+
+// decompress_host with the container and the content in device memory: index on the device, decode into the thread's slot
+// scratch, then one launch packs the blocks into d_dst.  Every verdict is in before the packing, so an error writes nothing.
+int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t n, uint8_t* d_dst, size_t dst_capacity, int single,
+                                const uint64_t* frame_hint, size_t nhint, size_t* src_consumed, void* stream)
+{
+    if (!d_dst && dst_capacity) return fail_arg("null pointer");
+    int err = 0; uint64_t slot_bytes = 0;
+    void* index = b200lz4f_index_create_dev(d_src, n, single, frame_hint, nhint, &slot_bytes, src_consumed, &err, stream);
+    if (!index) return err;
+    const FrameIndex& ix = *(const FrameIndex*)index;
+    const cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> blen(ix.blocks.size());
+    FrameReadScratch* s;
+    int64_t rc = get_frame_read_scratch(&s);
+    if (!rc) rc = reserve_device(s->d_slots, s->slots_cap, slot_bytes + 16);
+    if (!rc) rc = b200lz4f_decode_dev(index, d_src, s->d_slots, nullptr, nullptr, blen.data(), st);
+    if (rc >= 0 || rc == -11) {
+        uint64_t total = 0;
+        for (const int32_t l : blen) total += (uint64_t)l;
+        rc = total > dst_capacity ? -9 : reserve_device(s->d_pack, s->pack_cap, pack_desc_bytes(blen.size()));
+        if (!rc) {
+            cudaError_t e = pack_blocks(ix, blen.data(), s->d_slots, d_dst, s->d_pack, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+            rc = e == cudaSuccess ? (int64_t)total : fail_cuda(e, "packing the decoded blocks");
+        }
+    }
+    if (rc == B200LZ4_E_CUDA) cudaStreamSynchronize(st);
+    b200lz4f_index_free(index);
+    return rc;
+}
 
 } // extern "C"

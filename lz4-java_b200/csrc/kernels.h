@@ -90,6 +90,99 @@ cudaError_t launch_frame_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaS
 // every item: headers, block checksums, EndMarks, content checksums, f_off / f_end (frame_seal_kernel)
 cudaError_t launch_frame_seal(const FramePlan& p, cudaStream_t st);
 
+// ---- LZ4 Frame reader: the container walk (LZ4FrameInputStream.nextFrameInfo / readHeader / readBlock as an index pass,
+// LZ4FrameInputStream.java:132-321).  The host indexer (frame.cu) and the device one (frame_index.cu) both run walk_frames;
+// only where the facts go differs (the Sink).
+__host__ __device__ inline uint32_t rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
+
+// One frame as the walk found it.  At frame_begin: everything up to the header checksum byte; at frame_end: the rest.
+struct WalkFrame {
+    uint64_t desc_off, content_size, nblocks;
+    uint32_t content_checksum;
+    uint8_t flg, bd, hc_byte, desc_len;
+    bool complete, has_checksum, has_size;   // read up to its EndMark (and content checksum); the content checks that apply
+};
+struct WalkEnd { uint64_t ip; int err; bool seen, single_done; };   // where it stopped and why; seen: any frame, skippable ones too
+
+// Walks the frames of src[0, n) from ip, which must be where a frame (or a skippable frame) starts.  Stops at the first frame
+// boundary at or past stop_at, at the end of src, at the first malformed spot (err, -1 -2 -4 -10) or, with `single`, behind
+// the first non-skippable frame.  Bounds are checked against n, never stop_at.  Per frame the sink gets frame_begin, one
+// block(src_off, word, checksum) per complete block, and frame_end -- also for a frame the container breaks off inside
+// (complete = false).  Whether an error is the container's or the reader's is the caller's to say (it depends on what came
+// before ip).
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Sink>
+__host__ __device__ inline WalkEnd walk_frames(const uint8_t* src, uint64_t n, uint64_t ip, uint64_t stop_at, bool single, Sink& sink)
+{
+    WalkEnd e{ ip, 0, false, false };
+    while (ip < n && ip < stop_at) {
+        if (n - ip < 4) { e.err = -1; break; }
+        const uint32_t magic = rd32(src + ip); ip += 4;
+        if ((magic >> 4) == (0x184D2A50u >> 4)) {                               // skippable (:154,162-173)
+            if (n - ip < 4) { e.err = -1; break; }
+            const uint32_t sz = rd32(src + ip); ip += 4;
+            if (n - ip < sz) { e.err = -1; break; }
+            ip += sz; e.seen = true; continue;
+        }
+        if (magic != 0x184D2204u) { e.err = -2; break; }                        // (:151)
+        WalkFrame f{};
+        f.desc_off = ip;
+        if (n - ip < 3) { e.err = -1; break; }
+        f.flg = src[ip++]; f.bd = src[ip++];
+        if ((f.flg >> 6) != 1 || (f.flg & 2) || !(f.flg & 0x20) || (f.flg & 1)) { e.err = -10; break; }   // version, reserved, B.Indep, dictID
+        if ((f.bd & 0x8F) || (f.bd >> 4) < 4) { e.err = -10; break; }
+        const uint32_t bs = 1u << (8 + 2 * (f.bd >> 4));
+        f.has_size = f.flg & 8;
+        if (f.has_size) { if (n - ip < 9) { e.err = -1; break; } f.content_size = (uint64_t)rd32(src + ip) | ((uint64_t)rd32(src + ip + 4) << 32); ip += 8; }
+        if (n - ip < 1) { e.err = -1; break; }
+        f.desc_len = (uint8_t)(ip - f.desc_off);
+        f.hc_byte = src[ip++];
+        sink.frame_begin(f);
+        for (;;) {                                                              // readBlock (:258-321)
+            if (n - ip < 4) { e.err = -1; break; }
+            const uint32_t word = rd32(src + ip); ip += 4;
+            const uint32_t sz = word & 0x7FFFFFFFu;
+            if (sz == 0) break;                                                 // EndMark
+            if (sz > bs) { e.err = -4; break; }
+            const uint64_t at = ip;
+            if (n - ip < sz) { e.err = -1; break; }
+            ip += sz;
+            uint32_t sum = 0;
+            if (f.flg & 0x10) { if (n - ip < 4) { e.err = -1; break; } sum = rd32(src + ip); ip += 4; }
+            sink.block(at, word, sum);
+            f.nblocks++;
+        }
+        f.complete = !e.err;
+        f.has_checksum = !e.err && (f.flg & 4);
+        if (f.has_checksum) {
+            if (n - ip < 4) { e.err = -1; f.complete = false; f.has_checksum = false; }
+            else { f.content_checksum = rd32(src + ip); ip += 4; }
+        }
+        if (!f.complete) f.has_size = false;
+        sink.frame_end(f); e.seen = true;
+        if (single) { e.single_done = true; break; }                           // readSingleFrame (:83-91, 327, 346): the rest is not read
+        if (e.err) break;
+    }
+    e.ip = ip;
+    return e;
+}
+
+// The device walk (frame_index.cu): one thread per segment [seg_start, seg_end) of the container, records into a region of
+// its own.  A record is 16 bytes: a frame takes two (written at frame_end into the pair reserved at frame_begin), a block one;
+// they come in stream order.  A walker whose region is full keeps counting (WalkSummary.nrec) but stops writing.
+struct WalkSeg { uint64_t start, end, rec_off, rec_cap; };   // rec_off / rec_cap in records
+struct WalkSummary { uint64_t ip, nrec; int32_t err; uint32_t flags; };
+enum { WALK_SEEN = 1, WALK_SINGLE_DONE = 2 };
+struct WalkRec { uint64_t a, b; };
+// walkers [0, m): summaries, and lens[j] = the records walker j wrote (min(nrec, rec_cap))
+cudaError_t launch_frame_walk(const uint8_t* src, uint64_t n, bool single, const WalkSeg* segs, WalkSummary* sum, int32_t* lens,
+                              WalkRec* recs, uint32_t m, cudaStream_t st);
+// walker j's lens[j] records move from recs + segs[j].rec_off to packed + pos[j]
+cudaError_t launch_frame_pack(const WalkSeg* segs, const int32_t* lens, const uint64_t* pos, const WalkRec* recs, WalkRec* packed,
+                              uint32_t m, cudaStream_t st);
+
 // Average buffer length from which the hash batches give each buffer a whole warp (launch_xxh*_long) instead of a lane.
 static constexpr uint64_t XXH_LONG_AVG = 32768;
 
@@ -115,5 +208,15 @@ struct FrameScratch {
     cudaStream_t st2 = nullptr; cudaEvent_t fork = nullptr, join = nullptr;   // content checksums run beside the rest
 };
 int get_frame_scratch(FrameScratch** out);                 // selects the thread's device, like every entry point
+// Grow-or-keep scratch of the device frame reader (b200lz4f_index_create_dev / b200lz4f_decompress_dev), same lifetime.
+struct FrameReadScratch {
+    uint8_t* d_seg = nullptr; size_t seg_cap = 0;          // walker segments, summaries, record counts and positions
+    uint8_t* h_seg = nullptr; size_t h_seg_cap = 0;        // pinned: their upload, the summaries and the records coming back
+    uint8_t* d_recs = nullptr; size_t recs_cap = 0;        // the walkers' record regions
+    uint8_t* d_packed = nullptr; size_t packed_cap = 0;    // the records, packed for one copy back
+    uint8_t* d_slots = nullptr; size_t slots_cap = 0;      // decompress_dev: the decoded blocks, slot_bytes
+    uint8_t* d_pack = nullptr; size_t pack_cap = 0;        // decompress_dev: per-block descriptors of the final packing
+};
+int get_frame_read_scratch(FrameReadScratch** out);
 
 } // namespace b200

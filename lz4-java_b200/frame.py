@@ -112,6 +112,30 @@ def compress_frames_dev(src, src_off, src_len, block_size_code: int = 4, content
     return out[:r], frame_off, frame_len
 
 
+def decompress_frames_dev(src, max_decoded: int, read_single_frame: bool = False, frame_hints=None, out=None):
+    """decompress_frames for a container already in device memory, decoded into device memory (b200lz4f_decompress_dev):
+    no byte of the container or the content crosses to the host.  src: a contiguous uint8 CUDA tensor; out: a contiguous
+    uint8 CUDA tensor on src's device (default: a new one of max_decoded bytes); at most min(max_decoded, out.numel())
+    bytes are decoded.  frame_hints: offsets where frames are believed to start (compress_frames_dev's frame_off), which
+    lets the container be indexed in parallel; wrong hints cost time, never a different result.  Runs on torch's current
+    stream and returns out[:total] when it is written."""
+    import torch
+    if not isinstance(src, torch.Tensor) or src.dtype != torch.uint8 or not src.is_cuda or not src.is_contiguous():
+        raise ValueError("src must be a contiguous uint8 CUDA tensor")
+    if out is None:
+        out = torch.empty(max(max_decoded, 1), dtype=torch.uint8, device=src.device)
+    elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    hints = np.ascontiguousarray(np.asarray([] if frame_hints is None else frame_hints, dtype=np.uint64).reshape(-1))
+    r = N.lib().b200lz4f_decompress_dev(src.data_ptr(), src.numel(), out.data_ptr(), min(max_decoded, out.numel()),
+                                        int(bool(read_single_frame)), hints.ctypes.data if len(hints) else None, len(hints),
+                                        None, torch.cuda.current_stream(src.device).cuda_stream)
+    N.check(r)
+    if r < 0:
+        raise LZ4FrameError(int(r))
+    return out[:r]
+
+
 # ---- lz4-java's private "LZ4Block" container (LZ4BlockOutputStream / LZ4BlockInputStream)
 def compress_lz4block(src, block_size: int = 1 << 16, hc_level: int = 0) -> bytes:
     s = _view(src)
