@@ -224,6 +224,10 @@ int     b200lz4f_expected_content_size(const uint8_t* src, size_t srcSize, int64
 size_t  b200lz4f_index_frames(void* index);
 size_t  b200lz4f_index_blocks(void* index);
 void    b200lz4f_index_block_offsets(void* index, uint64_t* block_off);   /* b200lz4f_index_blocks() entries, bytes into d_slots */
+/* An index is host data, and decode_dev only reads it: several threads may decode one index at the same time, each into its
+ * own d_slots.  decode_dev runs on the calling thread's device, like every entry point: the one b200lz4_set_device chose,
+ * else the device current at the thread's first call into the library; d_src and d_slots are memory of that device.  Its
+ * descriptors and results go through scratch the thread keeps for its next calls.  b200lz4f_index_free makes no CUDA call. */
 int64_t b200lz4f_decode_dev(void* index, const uint8_t* d_src, uint8_t* d_slots, uint64_t* frame_off, uint64_t* frame_len,
                             int32_t* block_len_out, void* stream);
 void    b200lz4f_index_free(void* index);

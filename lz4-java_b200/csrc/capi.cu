@@ -34,7 +34,6 @@ int fail_cuda(cudaError_t e, const char* where)
     return tl_status = B200LZ4_E_CUDA;
 }
 int fail_arg(const char* what) { snprintf(tl_err, sizeof tl_err, "invalid argument: %s", what); return tl_status = B200LZ4_E_ARG; }
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail_cuda(e_, #call); } while (0)
 
 static int ensure_device()
 {
@@ -96,7 +95,8 @@ struct Ctx {
     // one-block path
     uint8_t* h_bounce = nullptr; size_t bounce_cap = 0;    // pinned: [src | dst]
     FrameScratch frame;                                    // b200lz4f_compress_dev (containers.cu)
-    FrameReadScratch frame_read;                           // b200lz4f_index_create_dev / b200lz4f_decompress_dev (frame.cu)
+    FrameReadScratch frame_read;                           // the frame reader (frame.cu)
+    SideStream side;                                       // both frame calls' checksum stream
     ~Ctx() { /* process teardown frees device memory; explicit frees would race CUDA shutdown */ }
 };
 
@@ -178,29 +178,39 @@ struct PipelineGuard {
     ~PipelineGuard() { if (!completed) ctx_abandon(c); }
 };
 
-int get_frame_scratch(FrameScratch** out)
+// the thread's context, with its side stream when `side` asks for it
+static int get_frame_ctx(Ctx** c, SideStream** side)
 {
-    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
-    FrameScratch& f = c->frame;
-    if (!f.st2) {
-        cudaError_t e = cudaStreamCreateWithFlags(&f.st2, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.fork, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.join, cudaEventDisableTiming);
+    int rc = get_ctx(c); if (rc) return rc;
+    if (!side) return 0;
+    SideStream& s = (*c)->side;
+    if (!s.st) {
+        cudaError_t e = cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming);
         if (e != cudaSuccess) {
-            if (f.st2) cudaStreamDestroy(f.st2);
-            if (f.fork) cudaEventDestroy(f.fork);
-            f.st2 = nullptr; f.fork = nullptr;
-            return fail_cuda(e, "creating the frame writer's checksum stream");
+            if (s.st) cudaStreamDestroy(s.st);
+            if (s.fork) cudaEventDestroy(s.fork);
+            s = SideStream{};
+            return fail_cuda(e, "creating the frame calls' checksum stream");
         }
     }
-    *out = &f;
+    *side = &s;
     return 0;
 }
 
-int get_frame_read_scratch(FrameReadScratch** out)
+int get_frame_scratch(FrameScratch** out, SideStream** side)
 {
-    Ctx* c; int rc = get_ctx(&c); if (rc) return rc;
+    Ctx* c; int rc = get_frame_ctx(&c, side); if (rc) return rc;
+    *out = &c->frame;
+    return 0;
+}
+
+int get_frame_read_scratch(FrameReadScratch** out, SideStream** side, cudaStream_t* idle)
+{
+    Ctx* c; int rc = get_frame_ctx(&c, side); if (rc) return rc;
     *out = &c->frame_read;
+    if (idle) *idle = c->slot[0].st;           // a pipeline call leaves its slots drained (run_pipeline, ctx_abandon)
     return 0;
 }
 

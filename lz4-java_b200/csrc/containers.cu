@@ -138,7 +138,7 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
     if (ni > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
     if (need > dst_capacity) return -9;
     if (too_long) return -10;                                       // the host writer's limit on a content checksum
-    FrameScratch* s; int rc = get_frame_scratch(&s); if (rc) return rc;
+    FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
     const FramePlanLayout L(nb, ni, nf);
     rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
     if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
@@ -184,43 +184,37 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
                        (uint32_t)ni, bsCode, flags };
     uint64_t* carry = (uint64_t*)(D + L.carry);
 
-    // ---- launches, all ordered after what `st` already holds.  A failure waits for what was queued: the scratch stays
-    // the thread's, and the next call may reuse or free it.
-    struct Drain {
-        cudaStream_t a, b; bool done = false;
-        ~Drain() { if (!done) { cudaStreamSynchronize(a); cudaStreamSynchronize(b); } }
-    } drain{ st, s->st2 };
-#define FCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail_cuda(e_, #call); } while (0)
+    // ---- launches, all ordered after what `st` already holds
+    Drain drain{ st, side->st };
     auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
-    FCK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
     if (flags & 1) {                // content checksums: the sources only, so from the start, beside everything else
-        FCK(cudaEventRecord(s->fork, st));
-        FCK(cudaStreamWaitEvent(s->st2, s->fork, 0));
-        FCK(counted(launch_xxh32_long(d_src, (const uint64_t*)(D + L.f_soff), (const int32_t*)(D + L.f_len32), 0,
-                                      (uint32_t*)(D + L.f_sum), nf, s->st2)));
-        FCK(cudaEventRecord(s->join, s->st2));
+        CK(cudaEventRecord(side->fork, st));
+        CK(cudaStreamWaitEvent(side->st, side->fork, 0));
+        CK(counted(launch_xxh32_long(d_src, (const uint64_t*)(D + L.f_soff), (const int32_t*)(D + L.f_len32), 0,
+                                     (uint32_t*)(D + L.f_sum), nf, side->st)));
+        CK(cudaEventRecord(side->join, side->st));
     }
     for (size_t k = 0; k < chunks.size(); k++) {
         const FrameChunk& c = chunks[k];
         if (c.b1 > c.b0) {          // the host writer's compressor and dispatch (compress_blocks above)
             const BatchArgs a{ d_src, P.b_soff + c.b0, P.b_slen + c.b0, s->d_slots, P.b_slot + c.b0,
                                (const int32_t*)(D + L.b_ccap) + c.b0, (int32_t*)P.b_clen + c.b0, c.b1 - c.b0 };
-            FCK(counted(hc_level > 0 ? launch_compress_hc(a, hc_level, st) : launch_compress_fast(a, bs <= 65536 ? 65536 : 0, st)));
+            CK(counted(hc_level > 0 ? launch_compress_hc(a, hc_level, st) : launch_compress_fast(a, bs <= 65536 ? 65536 : 0, st)));
         }
         const uint32_t i0 = (uint32_t)c.i0, n = (uint32_t)(c.i1 - c.i0);
-        FCK(counted(launch_frame_sizes(P, i0, n, st)));
-        FCK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
-        FCK(counted(launch_frame_emit(P, i0, n, st)));
+        CK(counted(launch_frame_sizes(P, i0, n, st)));
+        CK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
+        CK(counted(launch_frame_emit(P, i0, n, st)));
     }
     if ((flags & 2) && nb) {        // block checksums over the payloads as written; the source average bounds the payloads'
-        FCK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+        CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
             d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
     }
-    if (flags & 1) FCK(cudaStreamWaitEvent(st, s->join, 0));
-    FCK(counted(launch_frame_seal(P, st)));
-    FCK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
-    FCK(cudaStreamSynchronize(st));
-#undef FCK
+    if (flags & 1) CK(cudaStreamWaitEvent(st, side->join, 0));
+    CK(counted(launch_frame_seal(P, st)));
+    CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     drain.done = true;
     for (size_t f = 0; f < nf; f++) {
         if (frame_off) frame_off[f] = h64(L.f_off)[f];

@@ -22,6 +22,7 @@
 #endif
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -41,25 +42,38 @@ struct FrameRec {
 
 struct BlockRec { uint64_t src_off; uint32_t size; bool raw; uint32_t checksum; bool has_checksum; size_t frame; uint64_t out_off; uint32_t cap; };
 
+// Where decode_dev's descriptor arrays lie in one blob of nb blocks (nc compressed, nr stored) and nf frames, nbsum block
+// and nfsum content checksums; the same in the index, in d_seg and in h_seg.  The inputs come first and are uploaded, the
+// results last: each of them comes back.
+struct IndexLayout {
+    size_t c_soff, c_doff, c_slen, c_dcap;                  // compressed blocks
+    size_t r_soff, r_doff, r_len;                           // stored blocks
+    size_t h_off, h_len, b_off, b_len;                      // what the descriptor and block checksums hash
+    size_t f_first, f_nblk;                                 // content checksums (chained to the decoder: xxhash.cu)
+    size_t k_comp, k_rawlen, k_off;                         // per block: index among the compressed blocks (-1: stored), stored size, slot
+    size_t in, c_res, h_out, b_out, f_out, bytes = 0;       // in: the bytes of the inputs; then the results
+    IndexLayout(size_t nb, size_t nc, size_t nr, size_t nf, size_t nbsum, size_t nfsum)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        c_soff = take(8 * nc); c_doff = take(8 * nc); c_slen = take(4 * nc); c_dcap = take(4 * nc);
+        r_soff = take(8 * nr); r_doff = take(8 * nr); r_len = take(4 * nr);
+        h_off = take(8 * nf); h_len = take(4 * nf); b_off = take(8 * nbsum); b_len = take(4 * nbsum);
+        f_first = take(4 * nfsum); f_nblk = take(4 * nfsum);
+        k_comp = take(4 * nb); k_rawlen = take(4 * nb); k_off = take(8 * nb);
+        in = bytes;
+        c_res = take(4 * nc); h_out = take(4 * nf); b_out = take(4 * nbsum); f_out = take(4 * nfsum);
+    }
+};
+
+// Host data only: nothing writes to an index once build_descriptors has run, so any number of threads may decode it at once.
 struct FrameIndex {
     std::vector<FrameRec> frames;
     std::vector<BlockRec> blocks;
     uint64_t slot_bytes = 0;            // device bytes needed for the slot layout (upper bound of the decoded size)
     int tail_err = 0;                   // the container's own error, behind everything indexed (reported after what precedes it)
-    // device-side descriptor arrays, built once
-    int device = -1;
-    uint8_t* d_blob = nullptr; size_t blob_bytes = 0;
-    std::vector<uint8_t> h_blob;
-    // offsets inside the blob
-    size_t o_c_soff, o_c_doff, o_c_slen, o_c_dcap, o_c_res;          // compressed blocks
-    size_t o_r_soff, o_r_doff, o_r_len;                              // raw blocks
-    size_t o_h_off, o_h_len, o_h_out;                                // header descriptors
-    size_t o_b_off, o_b_len, o_b_out;                                // block checksums
-    size_t o_f_first, o_f_nblk, o_f_out;                                        // content checksums (chained to the decoder: xxhash.cu)
-    size_t o_k_comp, o_k_rawlen, o_k_off;                            // per block: index among the compressed blocks (-1: stored), stored size, slot
-    cudaStream_t st2 = nullptr; cudaEvent_t e1 = nullptr, e2 = nullptr;   // the checksum warps run beside the decoder
-    size_t n_comp = 0, n_raw = 0, n_bsum = 0, n_fsum = 0;
-    std::vector<size_t> comp_ix, raw_ix, bsum_ix, fsum_ix;
+    size_t n_comp = 0, n_raw = 0, n_bsum = 0, n_fsum = 0;      // compressed and stored blocks, block and content checksums
+    std::vector<uint8_t> blob;                                  // decode_dev's inputs, laid out by layout()
+    IndexLayout layout() const { return IndexLayout(blocks.size(), n_comp, n_raw, frames.size(), n_bsum, n_fsum); }
 };
 
 // The host sink of walk_frames (kernels.h): frames and blocks into the index, each block with its slot.  The device indexer
@@ -141,7 +155,6 @@ static int walk_segments(FrameReadScratch& s, const uint8_t* d_src, uint64_t n, 
     std::vector<size_t> todo(m);
     std::vector<uint64_t> cap(m);
     for (size_t j = 0; j < m; j++) { todo[j] = j; cap[j] = std::min(((end[j] - start[j]) >> 12) + 64, WALK_MAX_REC); }   // ~ one per 4 KiB
-#define WCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail_cuda(e_, #call); } while (0)
     while (!todo.empty()) {
         const size_t k = todo.size();
         const WalkLayout L(k);
@@ -156,22 +169,22 @@ static int walk_segments(FrameReadScratch& s, const uint8_t* d_src, uint64_t n, 
         uint64_t at = 0;
         for (size_t i = 0; i < k; i++) { const size_t j = todo[i]; hs[i] = WalkSeg{ start[j], end[j], at, cap[j] }; at += cap[j]; }
         uint8_t* D = s.d_seg;
-        WCK(cudaMemcpyAsync(D, s.h_seg, L.sums, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(D, s.h_seg, L.sums, cudaMemcpyHostToDevice, st));
         g_launch_count.fetch_add(3, std::memory_order_relaxed);
-        WCK(launch_frame_walk(d_src, n, single, (const WalkSeg*)D, (WalkSummary*)(D + L.sums), (int32_t*)(D + L.lens), (WalkRec*)s.d_recs, (uint32_t)k, st));
-        WCK(launch_scan((const int32_t*)(D + L.lens), (uint64_t*)(D + L.pos), (uint64_t*)(D + L.total), nullptr, k, st));
-        WCK(launch_frame_pack((const WalkSeg*)D, (const int32_t*)(D + L.lens), (const uint64_t*)(D + L.pos), (const WalkRec*)s.d_recs,
-                              (WalkRec*)s.d_packed, (uint32_t)k, st));
-        WCK(cudaMemcpyAsync(s.h_seg + L.sums, D + L.sums, L.bytes - L.sums, cudaMemcpyDeviceToHost, st));
-        WCK(cudaStreamSynchronize(st));
+        CK(launch_frame_walk(d_src, n, single, (const WalkSeg*)D, (WalkSummary*)(D + L.sums), (int32_t*)(D + L.lens), (WalkRec*)s.d_recs, (uint32_t)k, st));
+        CK(launch_scan((const int32_t*)(D + L.lens), (uint64_t*)(D + L.pos), (uint64_t*)(D + L.total), nullptr, k, st));
+        CK(launch_frame_pack((const WalkSeg*)D, (const int32_t*)(D + L.lens), (const uint64_t*)(D + L.pos), (const WalkRec*)s.d_recs,
+                             (WalkRec*)s.d_packed, (uint32_t)k, st));
+        CK(cudaMemcpyAsync(s.h_seg + L.sums, D + L.sums, L.bytes - L.sums, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
         const uint64_t packed = *(const uint64_t*)(s.h_seg + L.total);
         const WalkSummary* hsum = (const WalkSummary*)(s.h_seg + L.sums);
         const uint64_t* hpos = (const uint64_t*)(s.h_seg + L.pos);
         std::vector<WalkSummary> got(hsum, hsum + k);
         std::vector<uint64_t> pos(hpos, hpos + k);
         if (packed) {
-            WCK(cudaMemcpyAsync(s.h_seg, s.d_packed, packed * sizeof(WalkRec), cudaMemcpyDeviceToHost, st));
-            WCK(cudaStreamSynchronize(st));
+            CK(cudaMemcpyAsync(s.h_seg, s.d_packed, packed * sizeof(WalkRec), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
         }
         const size_t base = recs.size();
         recs.insert(recs.end(), (const WalkRec*)s.h_seg, (const WalkRec*)s.h_seg + packed);
@@ -186,7 +199,6 @@ static int walk_segments(FrameReadScratch& s, const uint8_t* d_src, uint64_t n, 
         }
         todo.swap(again);
     }
-#undef WCK
     return 0;
 }
 
@@ -239,74 +251,57 @@ static int index_frames_dev(FrameReadScratch& s, const uint8_t* d_src, uint64_t 
 }
 
 // Packs decoded blocks back to back: block b's blen[b] bytes move from d_slots + its slot to d_dst + the lengths before it.
-// d_desc: device room for pack_desc_bytes(blocks) of descriptors.  One launch; ordered on st.
-static size_t pack_desc_bytes(size_t nb) { return 2 * ((nb * 8 + 15) & ~size_t(15)) + nb * 4; }
-static cudaError_t pack_blocks(const FrameIndex& ix, const int32_t* blen, const uint8_t* d_slots, uint8_t* d_dst, uint8_t* d_desc, cudaStream_t st)
+// The descriptors go up through d_seg / h_seg, free again once decode_dev has returned.  One launch; ordered on st.
+static int pack_blocks(FrameReadScratch& s, const FrameIndex& ix, const int32_t* blen, const uint8_t* d_slots, uint8_t* d_dst, cudaStream_t st)
 {
     const size_t nb = ix.blocks.size();
-    if (nb == 0) return cudaSuccess;
-    const size_t o_to = (nb * 8 + 15) & ~size_t(15), o_len = 2 * o_to;
-    std::vector<uint8_t> h(pack_desc_bytes(nb));
+    if (nb == 0) return 0;
+    const size_t o_to = (nb * 8 + 15) & ~size_t(15), o_len = 2 * o_to, bytes = o_len + nb * 4;
+    int rc = reserve_device(s.d_seg, s.seg_cap, bytes);
+    if (!rc) rc = reserve_pinned(s.h_seg, s.h_seg_cap, bytes);
+    if (rc) return rc;
+    uint8_t* h = s.h_seg;
     uint64_t pos = 0;
     for (size_t b = 0; b < nb; b++) {
-        ((uint64_t*)h.data())[b] = ix.blocks[b].out_off;
-        ((uint64_t*)(h.data() + o_to))[b] = pos; pos += (uint64_t)blen[b];
+        ((uint64_t*)h)[b] = ix.blocks[b].out_off;
+        ((uint64_t*)(h + o_to))[b] = pos; pos += (uint64_t)blen[b];
     }
-    memcpy(h.data() + o_len, blen, nb * 4);
-    const cudaError_t e = cudaMemcpyAsync(d_desc, h.data(), h.size(), cudaMemcpyHostToDevice, st);   // pageable: staged before it returns
-    if (e != cudaSuccess) return e;
+    memcpy(h + o_len, blen, nb * 4);
+    CK(cudaMemcpyAsync(s.d_seg, h, bytes, cudaMemcpyHostToDevice, st));
     g_launch_count += 1;
-    return launch_gather(d_slots, (const uint64_t*)d_desc, (const int32_t*)(d_desc + o_len), d_dst, (const uint64_t*)(d_desc + o_to), nb, st);
-}
-
-template <typename T> static size_t put(std::vector<uint8_t>& blob, size_t count)
-{
-    size_t o = (blob.size() + 15) & ~size_t(15);
-    blob.resize(o + count * sizeof(T));
-    return o;
+    CK(launch_gather(d_slots, (const uint64_t*)s.d_seg, (const int32_t*)(s.d_seg + o_len), d_dst, (const uint64_t*)(s.d_seg + o_to), nb, st));
+    return 0;
 }
 
 static int build_descriptors(FrameIndex& ix)
 {
-    for (size_t i = 0; i < ix.blocks.size(); i++) {
-        (ix.blocks[i].raw ? ix.raw_ix : ix.comp_ix).push_back(i);
-        if (ix.blocks[i].has_checksum) ix.bsum_ix.push_back(i);
+    for (const BlockRec& b : ix.blocks) { (b.raw ? ix.n_raw : ix.n_comp)++; ix.n_bsum += b.has_checksum; }
+    for (const FrameRec& f : ix.frames) ix.n_fsum += f.has_checksum;
+    const IndexLayout L = ix.layout();
+    ix.blob.assign(L.in, 0);
+    uint8_t* p = ix.blob.data();
+    auto u64 = [&](size_t o) { return (uint64_t*)(p + o); };
+    auto i32 = [&](size_t o) { return (int32_t*)(p + o); };
+    size_t c = 0, r = 0, k = 0;
+    for (size_t b = 0; b < ix.blocks.size(); b++) {
+        const BlockRec& br = ix.blocks[b];
+        u64(L.k_off)[b] = br.out_off;
+        if (br.raw) {
+            i32(L.k_comp)[b] = -1; i32(L.k_rawlen)[b] = (int32_t)br.size;
+            u64(L.r_soff)[r] = br.src_off; u64(L.r_doff)[r] = br.out_off; i32(L.r_len)[r++] = (int32_t)br.size;
+        } else {
+            i32(L.k_comp)[b] = (int32_t)c;
+            u64(L.c_soff)[c] = br.src_off; u64(L.c_doff)[c] = br.out_off; i32(L.c_slen)[c] = (int32_t)br.size; i32(L.c_dcap)[c++] = (int32_t)br.cap;
+        }
+        if (br.has_checksum) { u64(L.b_off)[k] = br.src_off; i32(L.b_len)[k++] = (int32_t)br.size; }
     }
-    for (size_t f = 0; f < ix.frames.size(); f++) if (ix.frames[f].has_checksum) ix.fsum_ix.push_back(f);
-    ix.n_comp = ix.comp_ix.size(); ix.n_raw = ix.raw_ix.size(); ix.n_bsum = ix.bsum_ix.size(); ix.n_fsum = ix.fsum_ix.size();
-    auto& B = ix.h_blob;
-    const size_t nf = ix.frames.size();
-    ix.o_c_soff = put<uint64_t>(B, ix.n_comp); ix.o_c_doff = put<uint64_t>(B, ix.n_comp);
-    ix.o_c_slen = put<int32_t>(B, ix.n_comp);  ix.o_c_dcap = put<int32_t>(B, ix.n_comp); ix.o_c_res = put<int32_t>(B, ix.n_comp);
-    ix.o_r_soff = put<uint64_t>(B, ix.n_raw);  ix.o_r_doff = put<uint64_t>(B, ix.n_raw); ix.o_r_len = put<int32_t>(B, ix.n_raw);
-    ix.o_h_off = put<uint64_t>(B, nf); ix.o_h_len = put<int32_t>(B, nf); ix.o_h_out = put<uint32_t>(B, nf);
-    ix.o_b_off = put<uint64_t>(B, ix.n_bsum); ix.o_b_len = put<int32_t>(B, ix.n_bsum); ix.o_b_out = put<uint32_t>(B, ix.n_bsum);
-    ix.o_f_first = put<uint32_t>(B, ix.n_fsum); ix.o_f_nblk = put<uint32_t>(B, ix.n_fsum); ix.o_f_out = put<uint32_t>(B, ix.n_fsum);
-    ix.o_k_comp = put<int32_t>(B, ix.blocks.size()); ix.o_k_rawlen = put<int32_t>(B, ix.blocks.size());
-    ix.o_k_off = put<uint64_t>(B, ix.blocks.size());
-    B.resize((B.size() + 15) & ~size_t(15));
-    uint8_t* p = B.data();
-    for (size_t k = 0; k < ix.blocks.size(); k++) ((uint64_t*)(p + ix.o_k_off))[k] = ix.blocks[k].out_off;
-    for (size_t k = 0; k < ix.n_comp; k++) ((int32_t*)(p + ix.o_k_comp))[ix.comp_ix[k]] = (int32_t)k;
-    for (size_t k = 0; k < ix.n_raw; k++) { ((int32_t*)(p + ix.o_k_comp))[ix.raw_ix[k]] = -1; ((int32_t*)(p + ix.o_k_rawlen))[ix.raw_ix[k]] = (int32_t)ix.blocks[ix.raw_ix[k]].size; }
-    for (size_t k = 0; k < ix.n_fsum; k++) {
-        const FrameRec& fr = ix.frames[ix.fsum_ix[k]];
+    k = 0;
+    for (size_t f = 0; f < ix.frames.size(); f++) {
+        const FrameRec& fr = ix.frames[f];
+        u64(L.h_off)[f] = fr.desc_off; i32(L.h_len)[f] = fr.desc_len;
+        if (!fr.has_checksum) continue;
         if (fr.first_block > 0xFFFFFFFFull || fr.nblocks > 0xFFFFFFFFull) return -10;
-        ((uint32_t*)(p + ix.o_f_first))[k] = (uint32_t)fr.first_block; ((uint32_t*)(p + ix.o_f_nblk))[k] = (uint32_t)fr.nblocks;
-    }
-    for (size_t k = 0; k < ix.n_comp; k++) {
-        const BlockRec& b = ix.blocks[ix.comp_ix[k]];
-        ((uint64_t*)(p + ix.o_c_soff))[k] = b.src_off; ((uint64_t*)(p + ix.o_c_doff))[k] = b.out_off;
-        ((int32_t*)(p + ix.o_c_slen))[k] = (int32_t)b.size; ((int32_t*)(p + ix.o_c_dcap))[k] = (int32_t)b.cap;
-    }
-    for (size_t k = 0; k < ix.n_raw; k++) {
-        const BlockRec& b = ix.blocks[ix.raw_ix[k]];
-        ((uint64_t*)(p + ix.o_r_soff))[k] = b.src_off; ((uint64_t*)(p + ix.o_r_doff))[k] = b.out_off; ((int32_t*)(p + ix.o_r_len))[k] = (int32_t)b.size;
-    }
-    for (size_t f = 0; f < nf; f++) { ((uint64_t*)(p + ix.o_h_off))[f] = ix.frames[f].desc_off; ((int32_t*)(p + ix.o_h_len))[f] = ix.frames[f].desc_len; }
-    for (size_t k = 0; k < ix.n_bsum; k++) {
-        const BlockRec& b = ix.blocks[ix.bsum_ix[k]];
-        ((uint64_t*)(p + ix.o_b_off))[k] = b.src_off; ((int32_t*)(p + ix.o_b_len))[k] = (int32_t)b.size;
+        ((uint32_t*)(p + L.f_first))[k] = (uint32_t)fr.first_block; ((uint32_t*)(p + L.f_nblk))[k++] = (uint32_t)fr.nblocks;
     }
     return 0;
 }
@@ -392,102 +387,93 @@ int b200lz4f_expected_content_size(const uint8_t* src, size_t n, int64_t* conten
     }
 }
 
-void b200lz4f_index_free(void* index)
-{
-    FrameIndex* ix = (FrameIndex*)index;
-    if (!ix) return;
-    if (ix->d_blob) { cudaSetDevice(ix->device); cudaFree(ix->d_blob); }
-    if (ix->st2) { cudaSetDevice(ix->device); cudaStreamDestroy(ix->st2); cudaEventDestroy(ix->e1); cudaEventDestroy(ix->e2); }
-    delete ix;
-}
+void b200lz4f_index_free(void* index) { delete (FrameIndex*)index; }
 
 // Decode every indexed frame: d_src holds the container bytes, d_slots (>= slot_bytes) receives block b at its slot
 // (b200lz4f_index_block_offsets; full blocks of one frame lie back to back).  On success frame_off[f] / frame_len[f] (host
 // arrays, may be NULL) describe each frame's content, one run inside d_slots when no block was flushed short mid-frame;
 // otherwise -11 is returned after every check has passed and the caller reads block by block (the host path below does).
+// The descriptors go up from, and the results come back into, the thread's reader scratch: the index is only read.
 // Returns total decoded bytes or a negative code.
 int64_t b200lz4f_decode_dev(void* index, const uint8_t* d_src, uint8_t* d_slots, uint64_t* frame_off, uint64_t* frame_len,
                             int32_t* block_len_out, void* stream)
 {
-    FrameIndex& ix = *(FrameIndex*)index;
-    cudaStream_t st = (cudaStream_t)stream;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return B200LZ4_E_NODEVICE;
-    if (ix.st2 && ix.device != dev) { cudaSetDevice(ix.device); cudaStreamDestroy(ix.st2); cudaEventDestroy(ix.e1); cudaEventDestroy(ix.e2); cudaSetDevice(dev); ix.st2 = nullptr; }
-    if (!ix.d_blob || ix.device != dev) {
-        if (ix.d_blob) { cudaSetDevice(ix.device); cudaFree(ix.d_blob); cudaSetDevice(dev); ix.d_blob = nullptr; }
-        if (cudaMalloc(&ix.d_blob, ix.h_blob.size() + 16) != cudaSuccess) return B200LZ4_E_CUDA;
-        ix.device = dev;
-    }
-    if (!ix.st2) {
-        if (cudaStreamCreateWithFlags(&ix.st2, cudaStreamNonBlocking) != cudaSuccess) { ix.st2 = nullptr; return B200LZ4_E_CUDA; }
-        if (cudaEventCreateWithFlags(&ix.e1, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ix.e2, cudaEventDisableTiming) != cudaSuccess)
-            return B200LZ4_E_CUDA;
-    }
-    uint8_t* D = ix.d_blob; uint8_t* H = ix.h_blob.data();
+    const FrameIndex& ix = *(const FrameIndex*)index;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const IndexLayout L = ix.layout();
+    FrameReadScratch* s; SideStream* side;
+    int rc = get_frame_read_scratch(&s, &side);
+    if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes + 16);
+    if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
+    if (rc) return rc;
+    uint8_t *D = s->d_seg, *H = s->h_seg;
     const size_t nf = ix.frames.size();
-    if (cudaMemcpyAsync(D, H, ix.h_blob.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return B200LZ4_E_CUDA;
-    if (ix.n_comp && cudaMemsetAsync(D + ix.o_c_res, 0x80, ix.n_comp * 4, st) != cudaSuccess) return B200LZ4_E_CUDA;   // FRAME_RES_PENDING
+    std::copy(ix.blob.begin(), ix.blob.end(), H);
+    Drain drain{ st, side->st };
+    CK(cudaMemcpyAsync(D, H, L.in, cudaMemcpyHostToDevice, st));
+    if (ix.n_comp) CK(cudaMemsetAsync(D + L.c_res, 0x80, ix.n_comp * 4, st));       // FRAME_RES_PENDING
     // 1. header + block checksums
     g_launch_count += 1;
-    if (launch_xxh32(d_src, (uint64_t*)(D + ix.o_h_off), (int32_t*)(D + ix.o_h_len), 0, (uint32_t*)(D + ix.o_h_out), nf, st) != cudaSuccess) return B200LZ4_E_CUDA;
+    CK(launch_xxh32(d_src, (uint64_t*)(D + L.h_off), (int32_t*)(D + L.h_len), 0, (uint32_t*)(D + L.h_out), nf, st));
     if (ix.n_bsum) {
         // few long payloads: one warp per stream; many short ones: one lane per buffer (xxhash.cu)
-        uint64_t sum = 0; for (size_t k = 0; k < ix.n_bsum; k++) sum += ix.blocks[ix.bsum_ix[k]].size;
+        uint64_t sum = 0; for (const BlockRec& b : ix.blocks) if (b.has_checksum) sum += b.size;
         g_launch_count += 1;
-        if ((sum / ix.n_bsum >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
-                d_src, (uint64_t*)(D + ix.o_b_off), (int32_t*)(D + ix.o_b_len), 0, (uint32_t*)(D + ix.o_b_out), ix.n_bsum, st) != cudaSuccess) return B200LZ4_E_CUDA;
+        CK((sum / ix.n_bsum >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+               d_src, (uint64_t*)(D + L.b_off), (int32_t*)(D + L.b_len), 0, (uint32_t*)(D + L.b_out), ix.n_bsum, st));
     }
     // 2. stored blocks are copied, then every compressed block is decoded; 3. one warp per frame folds the blocks into the
-    // content checksum as the decoder hands them over (second stream; the decode kernel is launched FIRST and waits for nobody)
+    // content checksum as the decoder hands them over (side stream; the decode kernel is launched FIRST and waits for nobody)
     if (ix.n_raw) {
         g_launch_count += 1;
-        if (launch_gather(d_src, (uint64_t*)(D + ix.o_r_soff), (int32_t*)(D + ix.o_r_len), d_slots, (uint64_t*)(D + ix.o_r_doff), ix.n_raw, st) != cudaSuccess) return B200LZ4_E_CUDA;
+        CK(launch_gather(d_src, (uint64_t*)(D + L.r_soff), (int32_t*)(D + L.r_len), d_slots, (uint64_t*)(D + L.r_doff), ix.n_raw, st));
     }
-    if (cudaEventRecord(ix.e1, st) != cudaSuccess) return B200LZ4_E_CUDA;
+    CK(cudaEventRecord(side->fork, st));
     if (ix.n_comp) {
-        BatchArgs a{ d_src, (uint64_t*)(D + ix.o_c_soff), (int32_t*)(D + ix.o_c_slen), d_slots, (uint64_t*)(D + ix.o_c_doff),
-                     (int32_t*)(D + ix.o_c_dcap), (int32_t*)(D + ix.o_c_res), ix.n_comp };
+        BatchArgs a{ d_src, (uint64_t*)(D + L.c_soff), (int32_t*)(D + L.c_slen), d_slots, (uint64_t*)(D + L.c_doff),
+                     (int32_t*)(D + L.c_dcap), (int32_t*)(D + L.c_res), ix.n_comp };
         g_launch_count += 1;
-        if (launch_decompress_safe(a, st) != cudaSuccess) return B200LZ4_E_CUDA;
+        CK(launch_decompress_safe(a, st));
     }
     if (ix.n_fsum) {
-        if (cudaStreamWaitEvent(ix.st2, ix.e1, 0) != cudaSuccess) return B200LZ4_E_CUDA;
+        CK(cudaStreamWaitEvent(side->st, side->fork, 0));
         g_launch_count += 1;
-        if (launch_xxh32_frames_chained(d_slots, (uint64_t*)(D + ix.o_k_off), (uint32_t*)(D + ix.o_f_first), (uint32_t*)(D + ix.o_f_nblk),
-                                        (int32_t*)(D + ix.o_k_comp), (int32_t*)(D + ix.o_k_rawlen),
-                                        (int32_t*)(D + ix.o_c_res), (uint32_t*)(D + ix.o_f_out), ix.n_fsum, ix.st2) != cudaSuccess) return B200LZ4_E_CUDA;
-        if (cudaEventRecord(ix.e2, ix.st2) != cudaSuccess || cudaStreamWaitEvent(st, ix.e2, 0) != cudaSuccess) return B200LZ4_E_CUDA;
+        CK(launch_xxh32_frames_chained(d_slots, (uint64_t*)(D + L.k_off), (uint32_t*)(D + L.f_first), (uint32_t*)(D + L.f_nblk),
+                                       (int32_t*)(D + L.k_comp), (int32_t*)(D + L.k_rawlen), (int32_t*)(D + L.c_res),
+                                       (uint32_t*)(D + L.f_out), ix.n_fsum, side->st));
+        CK(cudaEventRecord(side->join, side->st));
+        CK(cudaStreamWaitEvent(st, side->join, 0));
     }
-    if (ix.n_comp && cudaMemcpyAsync(H + ix.o_c_res, D + ix.o_c_res, ix.n_comp * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return B200LZ4_E_CUDA;
-    if (cudaMemcpyAsync(H + ix.o_h_out, D + ix.o_h_out, nf * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return B200LZ4_E_CUDA;
-    if (ix.n_bsum && cudaMemcpyAsync(H + ix.o_b_out, D + ix.o_b_out, ix.n_bsum * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return B200LZ4_E_CUDA;
-    if (ix.n_fsum && cudaMemcpyAsync(H + ix.o_f_out, D + ix.o_f_out, ix.n_fsum * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) return B200LZ4_E_CUDA;
-    if (cudaStreamSynchronize(st) != cudaSuccess) return B200LZ4_E_CUDA;
+    if (ix.n_comp) CK(cudaMemcpyAsync(H + L.c_res, D + L.c_res, ix.n_comp * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(H + L.h_out, D + L.h_out, nf * 4, cudaMemcpyDeviceToHost, st));
+    if (ix.n_bsum) CK(cudaMemcpyAsync(H + L.b_out, D + L.b_out, ix.n_bsum * 4, cudaMemcpyDeviceToHost, st));
+    if (ix.n_fsum) CK(cudaMemcpyAsync(H + L.f_out, D + L.f_out, ix.n_fsum * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
 
     // the verdict, in the order the stream reader meets things: frame by frame -- descriptor hash (:208-216), then block by
-    // block its checksum (:298-303) and its decode (:307-311), then at the EndMark content checksum (:266-269) and size (:270-272)
-    std::vector<int32_t> bsum_of(ix.blocks.size(), -1), fsum_of(nf, -1);
-    for (size_t k = 0; k < ix.n_bsum; k++) bsum_of[ix.bsum_ix[k]] = (int32_t)k;
-    for (size_t k = 0; k < ix.n_fsum; k++) fsum_of[ix.fsum_ix[k]] = (int32_t)k;
-    const int32_t* blk_comp = (const int32_t*)(H + ix.o_k_comp);
+    // block its checksum (:298-303) and its decode (:307-311), then at the EndMark content checksum (:266-269) and size
+    // (:270-272).  Each kind of result is in block or frame order, so a running count finds the next one.
+    const uint32_t *h_out = (const uint32_t*)(H + L.h_out), *b_out = (const uint32_t*)(H + L.b_out), *f_out = (const uint32_t*)(H + L.f_out);
+    const int32_t* c_res = (const int32_t*)(H + L.c_res);
+    size_t kc = 0, kb = 0, kf = 0;
     std::vector<int32_t> blen(ix.blocks.size());
     int64_t total = 0; bool gaps = false;
     for (size_t f = 0; f < nf; f++) {
         const FrameRec& fr = ix.frames[f];
-        if (((((uint32_t*)(H + ix.o_h_out))[f] >> 8) & 0xFF) != fr.hc_byte) return -3;
+        if (((h_out[f] >> 8) & 0xFF) != fr.hc_byte) return -3;
         uint64_t len = 0;
         for (size_t k = 0; k < fr.nblocks; k++) {
             const size_t b = fr.first_block + k;
             const BlockRec& br = ix.blocks[b];
-            if (bsum_of[b] >= 0 && ((uint32_t*)(H + ix.o_b_out))[bsum_of[b]] != br.checksum) return -5;
+            if (br.has_checksum && b_out[kb++] != br.checksum) return -5;
             int32_t l = (int32_t)br.size;
-            if (!br.raw) { l = ((int32_t*)(H + ix.o_c_res))[blk_comp[b]]; if (l < 0) return -6; }   // LZ4Exception -> IOException
+            if (!br.raw) { l = c_res[kc++]; if (l < 0) return -6; }              // LZ4Exception -> IOException
             blen[b] = l;
             if (k + 1 < fr.nblocks && (uint32_t)l != fr.bs) gaps = true;          // a short block in the middle of a frame
             len += (uint64_t)l;
         }
-        if (fsum_of[f] >= 0 && ((uint32_t*)(H + ix.o_f_out))[fsum_of[f]] != fr.content_checksum) return -7;
+        if (fr.has_checksum && f_out[kf++] != fr.content_checksum) return -7;
         if (fr.has_size && fr.content_size != len) return -8;
         if (frame_off) frame_off[f] = fr.out_off;
         if (frame_len) frame_len[f] = len;
@@ -506,57 +492,41 @@ void b200lz4f_index_block_offsets(void* index, uint64_t* block_off)
     for (size_t b = 0; b < ix.blocks.size(); b++) block_off[b] = ix.blocks[b].out_off;
 }
 
-// Whole thing with HOST buffers: index, upload, decode, download frame by frame into one contiguous stream.
+// Whole thing with HOST buffers: index, upload, decode, download into one contiguous stream.  Runs on a stream of the thread's
+// context.  The container, the slots and the packed content are device memory of this call only, freed before it returns.
 static int64_t decompress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t dst_capacity, bool single, size_t* consumed)
 {
     int err = 0; uint64_t slot_bytes = 0;
-    void* index = index_create(src, n, single, &slot_bytes, consumed, &err);
-    if (!index) return err;
-    FrameIndex& ix = *(FrameIndex*)index;
-    int64_t rc = 0;
-    uint8_t *d_src = nullptr, *d_slots = nullptr;
-    cudaStream_t st = nullptr;
-    std::vector<uint64_t> foff(ix.frames.size()), flen(ix.frames.size());
-    std::vector<int32_t> blen(ix.blocks.size());
-    do {
-        if (b200lz4_device_count() <= 0) { rc = B200LZ4_E_NODEVICE; break; }
-        if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaMalloc(&d_src, n + 16) != cudaSuccess || cudaMalloc(&d_slots, slot_bytes + 16) != cudaSuccess) { rc = B200LZ4_E_CUDA; break; }
-        if (cudaMemcpyAsync(d_src, src, n, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = B200LZ4_E_CUDA; break; }
-        rc = b200lz4f_decode_dev(index, d_src, d_slots, foff.data(), flen.data(), blen.data(), st);
-        if (rc < 0 && rc != -11) break;
-        // download: per frame when contiguous, else per run of blocks (short blocks in the middle of a frame)
-        uint64_t pos = 0; bool ok = true;
-        if (rc >= 0) {
-            for (size_t f = 0; f < ix.frames.size() && ok; f++) {
-                if (pos + flen[f] > dst_capacity) { rc = -9; ok = false; break; }
-                if (flen[f] && cudaMemcpyAsync(dst + pos, d_slots + foff[f], flen[f], cudaMemcpyDeviceToHost, st) != cudaSuccess) { rc = B200LZ4_E_CUDA; ok = false; }
-                pos += flen[f];
-            }
-        } else {
-            // short blocks in mid-frame (everything is verified already): the device packs the blocks, one copy brings them back
-            rc = 0;
-            for (size_t b = 0; b < ix.blocks.size(); b++) pos += (uint64_t)blen[b];
-            if (pos > dst_capacity) { rc = -9; ok = false; }
-            uint8_t* d_tmp = nullptr;
-            const size_t o_out = (pack_desc_bytes(ix.blocks.size()) + 15) & ~size_t(15);
-            if (ok && pos) {
-                if (cudaMalloc(&d_tmp, o_out + pos + 16) != cudaSuccess) { rc = B200LZ4_E_CUDA; ok = false; d_tmp = nullptr; }
-                if (ok) {
-                    if (pack_blocks(ix, blen.data(), d_slots, d_tmp + o_out, d_tmp, st) != cudaSuccess ||
-                        cudaMemcpyAsync(dst, d_tmp + o_out, pos, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-                        cudaStreamSynchronize(st) != cudaSuccess) { rc = B200LZ4_E_CUDA; ok = false; }
-                }
-            }
-            if (d_tmp) cudaFree(d_tmp);
-        }
-        if (ok) { if (cudaStreamSynchronize(st) != cudaSuccess) rc = B200LZ4_E_CUDA; else rc = (int64_t)pos; }
-    } while (0);
-    if (d_src) cudaFree(d_src);
-    if (d_slots) cudaFree(d_slots);
-    if (st) cudaStreamDestroy(st);
-    b200lz4f_index_free(index);
-    return rc;
+    const std::unique_ptr<FrameIndex> ix((FrameIndex*)index_create(src, n, single, &slot_bytes, consumed, &err));
+    if (!ix) return err;
+    FrameReadScratch* s; cudaStream_t st;
+    int rc = get_frame_read_scratch(&s, nullptr, &st);
+    if (rc) return rc;
+    struct CallBuffer { uint8_t* p = nullptr; ~CallBuffer() { if (p) cudaFree(p); } } d_src, d_slots, d_out;
+    CK(cudaMalloc(&d_src.p, n + 16));
+    CK(cudaMalloc(&d_slots.p, slot_bytes + 16));
+    const size_t nf = ix->frames.size();
+    std::vector<uint64_t> foff(nf), flen(nf);
+    std::vector<int32_t> blen(ix->blocks.size());
+    Drain drain{ st };
+    CK(cudaMemcpyAsync(d_src.p, src, n, cudaMemcpyHostToDevice, st));
+    const int64_t got = b200lz4f_decode_dev(ix.get(), d_src.p, d_slots.p, foff.data(), flen.data(), blen.data(), st);
+    if (got < 0 && got != -11) return got;
+    uint64_t total = 0;
+    for (const int32_t l : blen) total += (uint64_t)l;
+    if (total > dst_capacity) return -9;
+    if (got >= 0) {                 // every frame is one run in the slots: one copy each
+        for (size_t f = 0, pos = 0; f < nf; pos += flen[f++])
+            if (flen[f]) CK(cudaMemcpyAsync(dst + pos, d_slots.p + foff[f], flen[f], cudaMemcpyDeviceToHost, st));
+    } else if (total) {             // short blocks mid-frame: the device packs the blocks, one copy brings them back
+        CK(cudaMalloc(&d_out.p, total + 16));
+        rc = pack_blocks(*s, *ix, blen.data(), d_slots.p, d_out.p, st);
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(dst, d_out.p, total, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    return (int64_t)total;
 }
 
 int64_t b200lz4f_decompress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t dst_capacity)
@@ -572,28 +542,25 @@ int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t n, uint8_t* d_dst, 
 {
     if (!d_dst && dst_capacity) return fail_arg("null pointer");
     int err = 0; uint64_t slot_bytes = 0;
-    void* index = b200lz4f_index_create_dev(d_src, n, single, frame_hint, nhint, &slot_bytes, src_consumed, &err, stream);
-    if (!index) return err;
-    const FrameIndex& ix = *(const FrameIndex*)index;
+    const std::unique_ptr<FrameIndex> ix((FrameIndex*)b200lz4f_index_create_dev(d_src, n, single, frame_hint, nhint, &slot_bytes,
+                                                                                 src_consumed, &err, stream));
+    if (!ix) return err;
     const cudaStream_t st = (cudaStream_t)stream;
-    std::vector<int32_t> blen(ix.blocks.size());
+    std::vector<int32_t> blen(ix->blocks.size());
     FrameReadScratch* s;
     int64_t rc = get_frame_read_scratch(&s);
     if (!rc) rc = reserve_device(s->d_slots, s->slots_cap, slot_bytes + 16);
-    if (!rc) rc = b200lz4f_decode_dev(index, d_src, s->d_slots, nullptr, nullptr, blen.data(), st);
-    if (rc >= 0 || rc == -11) {
-        uint64_t total = 0;
-        for (const int32_t l : blen) total += (uint64_t)l;
-        rc = total > dst_capacity ? -9 : reserve_device(s->d_pack, s->pack_cap, pack_desc_bytes(blen.size()));
-        if (!rc) {
-            cudaError_t e = pack_blocks(ix, blen.data(), s->d_slots, d_dst, s->d_pack, st);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-            rc = e == cudaSuccess ? (int64_t)total : fail_cuda(e, "packing the decoded blocks");
-        }
-    }
-    if (rc == B200LZ4_E_CUDA) cudaStreamSynchronize(st);
-    b200lz4f_index_free(index);
-    return rc;
+    if (!rc) rc = b200lz4f_decode_dev(ix.get(), d_src, s->d_slots, nullptr, nullptr, blen.data(), st);
+    if (rc < 0 && rc != -11) return rc;
+    uint64_t total = 0;
+    for (const int32_t l : blen) total += (uint64_t)l;
+    if (total > dst_capacity) return -9;
+    Drain drain{ st };
+    rc = pack_blocks(*s, *ix, blen.data(), s->d_slots, d_dst, st);
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    return (int64_t)total;
 }
 
 } // extern "C"

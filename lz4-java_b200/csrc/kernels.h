@@ -193,30 +193,42 @@ static inline uint64_t aligned_compress_bound(uint64_t len) { return (compress_b
 
 extern std::atomic<unsigned long long> g_launch_count;      // every kernel launch the library makes (any thread): b200lz4_launch_count()
 
-// ---- host layer shared by capi.cu and containers.cu
+// ---- host layer shared by capi.cu, containers.cu and frame.cu
 extern const size_t CHUNK_SPAN;                            // bytes of source per chunk of a chunked call (B200LZ4_CHUNK_MB, default 256)
 static constexpr size_t CHUNK_BLOCKS = 1 << 16;            // blocks per chunk at most
 int fail_arg(const char* what);                            // set the thread's error message, return B200LZ4_E_ARG
 int fail_cuda(cudaError_t e, const char* where);           // ... B200LZ4_E_CUDA or _NODEVICE
+// a failed CUDA call: the thread's error message names it, the caller returns fail_cuda's code
+#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return b200::fail_cuda(e_, #call); } while (0)
 int reserve_device(uint8_t*& p, size_t& cap, size_t need, int slack_shift = 2);   // grow-or-keep device buffer
 int reserve_pinned(uint8_t*& p, size_t& cap, size_t need);                       // grow-or-keep pinned buffer
+// A call that fails half way waits for what it queued on its streams: the scratch it used stays the thread's, and the next
+// call may reuse or free it.  Set done once the call has synchronised.
+struct Drain {
+    cudaStream_t a, b = nullptr; bool done = false;
+    ~Drain() { if (!done) { cudaStreamSynchronize(a); if (b) cudaStreamSynchronize(b); } }
+};
+// The frame calls' second stream, one per thread and device: the writer's content checksums and the reader's chained content
+// checksums run on it beside the caller's stream, from `fork` on, and every call joins it (`join`) before it returns.
+struct SideStream { cudaStream_t st = nullptr; cudaEvent_t fork = nullptr, join = nullptr; };
 // Grow-or-keep scratch of b200lz4f_compress_dev, one per thread and device (it lives in the thread's context).
 struct FrameScratch {
     uint8_t* d_plan = nullptr; size_t plan_cap = 0;        // the call's descriptors (FramePlan)
     uint8_t* h_plan = nullptr; size_t h_plan_cap = 0;      // pinned: their upload, and the results coming back
     uint8_t* d_slots = nullptr; size_t slots_cap = 0;      // one chunk's compressed blocks, bound-sized slots
-    cudaStream_t st2 = nullptr; cudaEvent_t fork = nullptr, join = nullptr;   // content checksums run beside the rest
 };
-int get_frame_scratch(FrameScratch** out);                 // selects the thread's device, like every entry point
-// Grow-or-keep scratch of the device frame reader (b200lz4f_index_create_dev / b200lz4f_decompress_dev), same lifetime.
+// Grow-or-keep scratch of the frame reader, same lifetime.  d_seg / h_seg serve every step in turn: the device walk, then
+// decode_dev's descriptors and results, then the packing descriptors.
 struct FrameReadScratch {
-    uint8_t* d_seg = nullptr; size_t seg_cap = 0;          // walker segments, summaries, record counts and positions
-    uint8_t* h_seg = nullptr; size_t h_seg_cap = 0;        // pinned: their upload, the summaries and the records coming back
+    uint8_t* d_seg = nullptr; size_t seg_cap = 0;          // walk: segments, summaries, counts, positions; decode: descriptors
+    uint8_t* h_seg = nullptr; size_t h_seg_cap = 0;        // pinned: their upload, and what comes back
     uint8_t* d_recs = nullptr; size_t recs_cap = 0;        // the walkers' record regions
     uint8_t* d_packed = nullptr; size_t packed_cap = 0;    // the records, packed for one copy back
     uint8_t* d_slots = nullptr; size_t slots_cap = 0;      // decompress_dev: the decoded blocks, slot_bytes
-    uint8_t* d_pack = nullptr; size_t pack_cap = 0;        // decompress_dev: per-block descriptors of the final packing
 };
-int get_frame_read_scratch(FrameReadScratch** out);
+// Both select the thread's device, like every entry point.  side (may be NULL): the side stream, created at its first use.
+// idle (may be NULL): a stream of the thread's context that no call keeps busy between calls.
+int get_frame_scratch(FrameScratch** out, SideStream** side);
+int get_frame_read_scratch(FrameReadScratch** out, SideStream** side = nullptr, cudaStream_t* idle = nullptr);
 
 } // namespace b200

@@ -366,6 +366,123 @@ def test_index_launches_do_not_depend_on_frames(b200, port):
         assert counts[0] == counts[1], (with_hints, counts)
 
 
+def test_freeing_an_index_leaves_the_current_device(b200, port, monkeypatch):
+    """an index decoded on device 1 and freed after the thread went back to device 0: the current device stays 0, because
+    freeing an index makes no CUDA call.  Two pretend devices on the emulator, two GPUs on a GPU box."""
+    L, M = b200._native.lib(), _DevMem()
+    if SIM:
+        if not hasattr(L, "b200lz4_sim_current_device"):
+            pytest.skip("this emulator library has no current-device accessor: tests/simt/copy_count.cpp")
+        monkeypatch.setenv("SIMT_DEVICES", "2")
+        current = L.b200lz4_sim_current_device
+    else:
+        import torch
+        if torch.cuda.device_count() < 2:
+            pytest.skip("needs two GPUs")
+        current = torch.cuda.current_device
+    data = port.datagen(100000, 0.5, 0.0, 12).tobytes()
+    blob = b200.compress_frame(data, 4, True, True, False)
+    ix, err, slot, _ = _index(L, M, blob, False, dev=False)
+    assert ix and err == 0
+    try:
+        assert L.b200lz4_set_device(1) == 0
+        d_src, d_slots = _src(M, blob), M.full(slot + 64, 0)              # memory of device 1, the current one now
+        assert L.b200lz4f_decode_dev(ix, M.ptr(d_src), M.ptr(d_slots), None, None, None, None) == len(data)
+        assert M.down(d_slots)[:len(data)].tobytes() == data
+        assert L.b200lz4_set_device(0) == 0
+        L.b200lz4f_index_free(ix)
+        assert current() == 0
+    finally:
+        L.b200lz4_set_device(0)
+
+
+def test_one_index_decoded_by_several_threads(b200, port):
+    """four threads decode one index at once, each into its own slots and on its own stream, many times over: every decode
+    gives what one thread alone gets (decode_dev only reads the index)"""
+    import threading
+    L, M = b200._native.lib(), _DevMem()
+    base = port.datagen(1 << 19, 0.5, 0.0, 13).tobytes()
+    frames = [b200.compress_frame(base[:n], 4, True, True, True) for n in ((70000, 1, 5000) if SIM else (3000000, 1, 70000))]
+    frames.append(_frame_of_pieces(port, [base[:5000], base[7:100], base[200:60000]], 4, block_checksum=True, stored={1}))
+    blob = SKIP.join(frames)
+    ix, err, slot, _ = _index(L, M, blob, False, dev=False)
+    assert ix and err == 0
+    nf, nb = L.b200lz4f_index_frames(ix), L.b200lz4f_index_blocks(ix)
+    d_src = _src(M, blob)
+    if not SIM:
+        import torch
+        torch.cuda.synchronize()
+
+    def decode(stream=None):
+        d_slots = M.full(slot + 64, 0)
+        if stream is not None:
+            stream.wait_stream(torch.cuda.current_stream())                  # the slots are filled on this thread's stream
+        fo, fl, bl = np.zeros(nf, dtype=np.uint64), np.zeros(nf, dtype=np.uint64), np.zeros(nb, dtype=np.int32)
+        rc = L.b200lz4f_decode_dev(ix, M.ptr(d_src), M.ptr(d_slots), fo.ctypes.data, fl.ctypes.data, bl.ctypes.data,
+                                   None if stream is None else stream.cuda_stream)
+        return rc, fo.tolist(), fl.tolist(), bl.tolist(), M.down(d_slots).tobytes()
+
+    want = decode()
+    assert want[0] == -11, want[0]
+    got = [[] for _ in range(4)]
+
+    def worker(k):
+        stream = None if SIM else torch.cuda.Stream()
+        for _ in range(3 if SIM else 30):
+            got[k].append(decode(stream))
+
+    threads = [threading.Thread(target=worker, args=(k,)) for k in range(4)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    L.b200lz4f_index_free(ix)
+    assert all(len(g) == (3 if SIM else 30) and all(r == want for r in g) for g in got), [[r[0] for r in g] for g in got]
+
+
+_FAILED_PINNED = r"""
+import ctypes, os, sys
+import numpy as np
+lib = ctypes.CDLL(sys.argv[1])
+vp = ctypes.c_void_p
+lib.b200lz4f_index_create.restype, lib.b200lz4f_index_create.argtypes = vp, [vp, ctypes.c_size_t, vp, vp]
+lib.b200lz4f_decode_dev.restype, lib.b200lz4f_decode_dev.argtypes = ctypes.c_int64, [vp] * 7
+lib.b200lz4f_index_free.argtypes = [vp]
+lib.b200lz4_last_error.restype = ctypes.c_char_p
+blob, data = (np.fromfile(f, dtype=np.uint8) for f in sys.argv[2:4])
+slot, err = ctypes.c_uint64(0), ctypes.c_int(0)
+ix = lib.b200lz4f_index_create(blob.ctypes.data, len(blob), ctypes.byref(slot), ctypes.byref(err))
+assert ix and err.value == 0, err.value
+d_src = np.concatenate([blob, np.zeros(64, dtype=np.uint8)])
+def decode():
+    d_slots, fo, fl = np.zeros(slot.value + 64, dtype=np.uint8), np.zeros(1, dtype=np.uint64), np.zeros(1, dtype=np.uint64)
+    rc = lib.b200lz4f_decode_dev(ix, d_src.ctypes.data, d_slots.ctypes.data, fo.ctypes.data, fl.ctypes.data, None, None)
+    return rc, d_slots[int(fo[0]):int(fo[0] + fl[0])]
+os.environ["SIMT_FAIL_HOST_ALLOC"] = "1"
+rc, _ = decode()                            # the thread's first decode: its pinned scratch cannot be allocated
+del os.environ["SIMT_FAIL_HOST_ALLOC"]
+assert rc == -2147483646 and b"cudaHostAlloc" in lib.b200lz4_last_error(), (rc, lib.b200lz4_last_error())
+rc, out = decode()
+assert rc == len(data) and out.tobytes() == data.tobytes(), rc
+lib.b200lz4f_index_free(ix)
+print("ok")
+"""
+
+
+@pytest.mark.skipif(not SIM, reason="the emulator build can make pinned allocations fail (SIMT_FAIL_HOST_ALLOC)")
+def test_failed_pinned_allocation_leaves_the_index_usable(b200, port, tmp_path):
+    """decode_dev whose pinned scratch cannot be allocated returns B200LZ4_E_CUDA and names cudaHostAlloc; the same index then
+    decodes correctly.  In a fresh process, whose thread has no pinned scratch yet."""
+    import subprocess
+    import sys
+    data = port.datagen(200000, 0.5, 0.0, 14).tobytes()
+    (tmp_path / "blob").write_bytes(b200.compress_frame(data, 4, True, True, False))
+    (tmp_path / "data").write_bytes(data)
+    r = subprocess.run([sys.executable, "-c", _FAILED_PINNED, os.environ["B200LZ4_TEST_SO"], str(tmp_path / "blob"), str(tmp_path / "data")],
+                       capture_output=True, text=True)
+    assert r.returncode == 0 and r.stdout.strip() == "ok", (r.returncode, r.stdout[-2000:] + r.stderr[-2000:])
+
+
 @pytest.mark.skipif(SIM, reason="torch streams: GPU only")
 def test_ordered_after_the_stream(b200, port):
     """the container is written by a torch op on a side stream and decompress_frames_dev is called on that stream without a

@@ -1,7 +1,7 @@
 """The device frame reader's tests (test_frame_decode_dev.py) on a box without a GPU: against the emulator build of the whole
 library, with 1 MiB chunks as for the device writer's tests.  The library is built here with the same sources and flags as
 tests/simt/build_sim_library.sh, plus tests/simt/copy_count.h force-included, so that the tests can also count the bytes
-the library copies between host and device."""
+the library copies between host and device, and read the stand-in runtime's current device."""
 import os
 import subprocess
 import sys
@@ -41,4 +41,4 @@ def test_device_frame_reader_on_the_emulator_library(counted_sim_library):
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(HERE, "test_frame_decode_dev.py"), "-m", "gpu", "-q", "-x",
                         "-p", "no:cacheprovider", "-W", "ignore::DeprecationWarning"],
                        env=env, cwd=ROOT, capture_output=True, text=True)
-    assert r.returncode == 0 and "8 passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+    assert r.returncode == 0 and "11 passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
