@@ -251,15 +251,16 @@ void*   b200lz4f_index_create_dev(const uint8_t* d_src, size_t srcSize, int sing
  * Ordered after the work already queued on `stream`; returns when d_dst holds the content. */
 int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t srcSize, uint8_t* d_dst, size_t dstCapacity, int single,
                                 const uint64_t* frame_hint, size_t nhint, size_t* src_consumed, void* stream);
-/* Device-resident LZ4 Frame writer (LZ4FrameOutputStream.java:178-251, as b200lz4f_compress_host_hc writes it) for nf
- * independent frames.  Frame f is src_len[f] bytes at d_src + src_off[f] (src_off / src_len: HOST arrays of nf entries; the
- * bytes are in device memory of the current device).  The frames are written back to back into d_dst (device, dst_capacity
- * bytes), each one byte for byte the frame b200lz4f_compress_host_hc would write for the same bytes at the same 16-byte
- * phase with the same bsCode / flags / hc_level; frame_off[f] / frame_len[f] (host, may be NULL) say where.  Ordered after
- * the work already queued on `stream`; returns when the frames are in d_dst.
+/* Device-resident LZ4 Frame writer (LZ4FrameOutputStream.java:178-251) for nf independent frames, with bsCode / flags /
+ * hc_level as b200lz4f_compress_host_hc takes them.  Frame f is src_len[f] bytes at d_src + src_off[f] (src_off / src_len:
+ * HOST arrays of nf entries; the bytes are in device memory of the current device).  The frames are written back to back
+ * into d_dst (device, dst_capacity bytes); frame_off[f] / frame_len[f] (host, may be NULL) say where.  b200lz4f_compress_host_hc
+ * is this writer run on a device copy of its source at the source's 16-byte phase, so each frame is byte for byte the one it
+ * writes for the same bytes at the same phase.  Ordered after the work already queued on `stream`; returns when the frames
+ * are in d_dst.
  * Returns the total bytes written, or: -9 dst_capacity < sum of b200lz4f_compress_bound(src_len[f], bsCode);
- * -10 content checksum requested for a frame longer than 0x7FFFFFFF bytes (the host writer's limit); B200LZ4_E_ARG, _CUDA,
- * _NODEVICE.  Argument and size errors are found before anything is launched or written. */
+ * -10 content checksum requested for a frame longer than 0x7FFFFFFF bytes; B200LZ4_E_ARG, _CUDA, _NODEVICE.  Argument and
+ * size errors are found before anything is launched or written. */
 int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
                               uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
                               int bsCode, int flags, int hc_level, void* stream);
@@ -272,6 +273,9 @@ int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, con
  * Length-prefixed blocks (LZ4CompressorWithLength / LZ4DecompressorWithLength).
  * Return: bytes written / decoded, or negative: -1 premature end, -2 corrupted, -9 dst too small, B200LZ4_E_*. */
 size_t  b200lz4f_compress_bound(size_t srcSize, int bsCode);
+/* The frame is written on the calling thread's device by b200lz4f_compress_dev, from a copy of src staged at src's 16-byte
+ * phase.  Besides b200lz4f_compress_dev's scratch, the call needs srcSize + b200lz4f_compress_bound(srcSize, bsCode) (plus up
+ * to 30) bytes of device memory for that copy and the frame, and the thread keeps them for its next calls. */
 int64_t b200lz4f_compress_host(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCapacity, int bsCode, int flags);
 /* the writers' LZ4Compressor argument (LZ4FrameOutputStream.java:132-133, LZ4BlockOutputStream.java:96,124): hc_level 0 = the
  * fast compressor (what the calls without _hc use), 1..17 = LZ4_compress_HC at that level */

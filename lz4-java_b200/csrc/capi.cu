@@ -94,7 +94,7 @@ struct Ctx {
     Slot slot[NSLOTS];
     // one-block path
     uint8_t* h_bounce = nullptr; size_t bounce_cap = 0;    // pinned: [src | dst]
-    FrameScratch frame;                                    // b200lz4f_compress_dev (containers.cu)
+    FrameScratch frame;                                    // the frame writer (containers.cu)
     FrameReadScratch frame_read;                           // the frame reader (frame.cu)
     SideStream side;                                       // both frame calls' checksum stream
     ~Ctx() { /* process teardown frees device memory; explicit frees would race CUDA shutdown */ }
@@ -199,10 +199,11 @@ static int get_frame_ctx(Ctx** c, SideStream** side)
     return 0;
 }
 
-int get_frame_scratch(FrameScratch** out, SideStream** side)
+int get_frame_scratch(FrameScratch** out, SideStream** side, cudaStream_t* idle)
 {
     Ctx* c; int rc = get_frame_ctx(&c, side); if (rc) return rc;
     *out = &c->frame;
+    if (idle) *idle = c->slot[0].st;           // a pipeline call leaves its slots drained (run_pipeline, ctx_abandon)
     return 0;
 }
 

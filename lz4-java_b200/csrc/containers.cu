@@ -4,9 +4,9 @@
 //   * "LZ4Block" container — LZ4BlockOutputStream.flushBufferedData/finish (:203-266) and
 //                            LZ4BlockInputStream.refill (LZ4BlockInputStream.java:191-264)
 //   * length-prefixed block — LZ4CompressorWithLength / LZ4DecompressorWithLength
-// The reference does these one block per native call; here the host only lays out headers and the
-// payload work (block compression / decompression, every XXH32) goes through the batch entry points,
-// i.e. the CUDA kernels.  No hashing or codec arithmetic runs on the host.
+// The reference does these one block per native call.  Here the frame is written on the device (frame_encode.cu), and the
+// LZ4Block container's host code only lays out headers while the payload work (block compression / decompression, every
+// XXH32) goes through the batch entry points, i.e. the CUDA kernels.  No hashing or codec arithmetic runs on the host.
 #include "../../include/b200lz4.h"
 #include "kernels.h"
 #ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device frame writer's kernels come with it
@@ -19,7 +19,7 @@
 static inline void put32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
 static inline uint32_t get32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
 
-// The writers' compressor argument (LZ4FrameOutputStream / LZ4BlockOutputStream take any LZ4Compressor): hc_level 0 = the fast
+// The LZ4Block writer's compressor argument (LZ4BlockOutputStream takes any LZ4Compressor): hc_level 0 = the fast
 // compressor, packed output; 1..17 = LZ4_compress_HC at that level into bound-sized slots.  coff/clen as *_compact_host.
 static int compress_blocks(const uint8_t* src, const uint64_t* soff, const int32_t* slen, uint8_t* tmp, size_t tmp_cap,
                            uint64_t* coff, int32_t* clen, size_t nb, int max_src_len, int hc_level)
@@ -35,66 +35,7 @@ static int compress_blocks(const uint8_t* src, const uint64_t* soff, const int32
     return b200lz4_compress_hc_batch_host(src, soff, slen, tmp, coff, ccap.data(), clen, nb, hc_level);
 }
 
-extern "C" {
-
-size_t b200lz4f_compress_bound(size_t n, int bsCode)
-{
-    if (bsCode < 4 || bsCode > 7) return 0;
-    const size_t bs = (size_t)1 << (8 + 2 * bsCode), nb = (n + bs - 1) / bs;
-    return 4 + 2 + 8 + 1 + nb * 8 + n + 4 + 4;
-}
-
-// flags: bit0 content checksum, bit1 block checksums, bit2 content size.  Returns bytes written or a negative code.
-int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags, int hc_level)
-{
-    if (bsCode < 4 || bsCode > 7) return B200LZ4_E_ARG;
-    if (cap < b200lz4f_compress_bound(n, bsCode)) return -9;
-    const size_t bs = (size_t)1 << (8 + 2 * bsCode), nb = (n + bs - 1) / bs;
-    size_t o = 0;
-    put32(dst, 0x184D2204u); o = 4;
-    const size_t hdr = o;
-    o += (size_t)b200::frame_descriptor(dst + o, bsCode, flags, n);
-    const uint32_t hh = b200xxh32(dst + hdr, o - hdr, 0);                        // descriptor checksum (:187)
-    if (hh == 0 && b200lz4_last_error()[0]) { /* a real zero hash is possible; device errors are caught below */ }
-    dst[o++] = (uint8_t)((hh >> 8) & 0xFF);
-    if (nb) {
-        std::vector<uint64_t> soff(nb), coff(nb), poff(nb);
-        std::vector<int32_t> slen(nb), clen(nb), plen(nb);
-        for (size_t i = 0; i < nb; i++) { soff[i] = i * bs; slen[i] = (int32_t)((n - i * bs) < bs ? (n - i * bs) : bs); }
-        size_t tmp_cap = 0; for (size_t i = 0; i < nb; i++) tmp_cap += (size_t)slen[i] + slen[i] / 255 + 32;
-        uint8_t* tmp = (uint8_t*)malloc(tmp_cap ? tmp_cap : 1);
-        if (!tmp) return B200LZ4_E_ARG;
-        int rc = compress_blocks(src, soff.data(), slen.data(), tmp, tmp_cap, coff.data(), clen.data(), nb, bs <= 65536 ? 65536 : 0, hc_level);
-        if (rc) { free(tmp); return rc; }
-        for (size_t i = 0; i < nb; i++) {                                        // writeBlock (:199-235)
-            const bool raw = clen[i] <= 0 || clen[i] >= slen[i];                 // stored uncompressed when it does not shrink (:215-222)
-            const uint32_t sz = raw ? (uint32_t)slen[i] : (uint32_t)clen[i];
-            put32(dst + o, sz | (raw ? 0x80000000u : 0u)); o += 4;
-            memcpy(dst + o, raw ? src + soff[i] : tmp + coff[i], sz);
-            poff[i] = o; plen[i] = (int32_t)sz; o += sz;
-            if (flags & 2) o += 4;                                               // block checksum slot, filled below
-        }
-        free(tmp);
-        if (flags & 2) {
-            std::vector<uint32_t> sums(nb);
-            rc = b200xxh32_batch_host(dst, poff.data(), plen.data(), 0, sums.data(), nb);
-            if (rc) return rc;
-            for (size_t i = 0; i < nb; i++) put32(dst + poff[i] + plen[i], sums[i]);
-        }
-    }
-    put32(dst + o, 0); o += 4;                                                   // EndMark (:243-245)
-    if (flags & 1) {
-        if (n > 0x7FFFFFFFull) return -10;
-        put32(dst + o, b200xxh32(src, n, 0)); o += 4;                            // content checksum (:246-249)
-    }
-    return (int64_t)o;
-}
-int64_t b200lz4f_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags)
-{ return b200lz4f_compress_host_hc(src, n, dst, cap, bsCode, flags, 0); }
-
-} // extern "C"
-
-// ---------------------------------------------------------------- LZ4 Frame writer, device memory (frame_encode.cu)
+// ---------------------------------------------------------------- LZ4 Frame writer (frame_encode.cu)
 namespace b200 {
 
 // Where the FramePlan arrays of a call with nb blocks, ni items and nf frames lie in one blob, the same on the host and the
@@ -137,7 +78,7 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
     if (bytes && !d_src) return fail_arg("null pointer");
     if (ni > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
     if (need > dst_capacity) return -9;
-    if (too_long) return -10;                                       // the host writer's limit on a content checksum
+    if (too_long) return -10;                                       // the content checksum kernel takes 31-bit lengths (f_len32)
     FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
     const FramePlanLayout L(nb, ni, nf);
     rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
@@ -197,7 +138,7 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
     }
     for (size_t k = 0; k < chunks.size(); k++) {
         const FrameChunk& c = chunks[k];
-        if (c.b1 > c.b0) {          // the host writer's compressor and dispatch (compress_blocks above)
+        if (c.b1 > c.b0) {          // the stream's compressor argument: hc_level 0 = the fast compressor, 1..17 = HC
             const BatchArgs a{ d_src, P.b_soff + c.b0, P.b_slen + c.b0, s->d_slots, P.b_slot + c.b0,
                                (const int32_t*)(D + L.b_ccap) + c.b0, (int32_t*)P.b_clen + c.b0, c.b1 - c.b0 };
             CK(counted(hc_level > 0 ? launch_compress_hc(a, hc_level, st) : launch_compress_fast(a, bs <= 65536 ? 65536 : 0, st)));
@@ -227,6 +168,13 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
 
 extern "C" {
 
+size_t b200lz4f_compress_bound(size_t n, int bsCode)
+{
+    if (bsCode < 4 || bsCode > 7) return 0;
+    const size_t bs = (size_t)1 << (8 + 2 * bsCode), nb = (n + bs - 1) / bs;
+    return 4 + 2 + 8 + 1 + nb * 8 + n + 4 + 4;
+}
+
 int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
                               uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
                               int bsCode, int flags, int hc_level, void* stream)
@@ -234,6 +182,30 @@ int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, con
     return b200::compress_frames_dev(d_src, src_off, src_len, nf, d_dst, dst_capacity, frame_off, frame_len, bsCode, flags,
                                      hc_level, (cudaStream_t)stream);
 }
+
+// The device writer on a copy of src in the thread's staging buffer: the source at its own 16-byte phase (the fast
+// compressor's chunks, and so its streams, follow the source's alignment), the frame behind it.
+int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags, int hc_level)
+{
+    if (bsCode < 4 || bsCode > 7) return b200::fail_arg("bsCode must be 4..7");
+    const size_t bound = b200lz4f_compress_bound(n, bsCode);
+    if (cap < bound) return -9;
+    b200::FrameScratch* s; cudaStream_t st;
+    int rc = b200::get_frame_scratch(&s, nullptr, &st); if (rc) return rc;
+    const uint64_t phase = (uintptr_t)src & 15, len = n, at = (phase + n + 15) & ~uint64_t(15);
+    rc = b200::reserve_device(s->d_stage, s->stage_cap, at + bound); if (rc) return rc;
+    b200::Drain drain{ st };
+    CK(cudaMemcpyAsync(s->d_stage + phase, src, n, cudaMemcpyHostToDevice, st));
+    const int64_t w = b200::compress_frames_dev(s->d_stage, &phase, &len, 1, s->d_stage + at, bound, nullptr, nullptr, bsCode,
+                                                flags, hc_level, st);
+    if (w < 0) return w;
+    CK(cudaMemcpyAsync(dst, s->d_stage + at, (size_t)w, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    return w;
+}
+int64_t b200lz4f_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags)
+{ return b200lz4f_compress_host_hc(src, n, dst, cap, bsCode, flags, 0); }
 
 // ---------------------------------------------------------------- "LZ4Block" container
 static const uint8_t LZ4BLOCK_MAGIC[8] = { 'L', 'Z', '4', 'B', 'l', 'o', 'c', 'k' };

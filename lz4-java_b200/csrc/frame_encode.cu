@@ -1,7 +1,8 @@
-// frame_encode.cu — the device half of the LZ4 Frame writer b200lz4f_compress_dev (containers.cu): what
-// LZ4FrameOutputStream.writeHeader / writeBlock / writeEndMark write (LZ4FrameOutputStream.java:178-251), for many frames
-// whose bytes are in device memory.  The host only plans (blocks, items, chunks: no payload byte is touched).  The blocks
-// are compressed by the library's batch compressors into bound-sized slots one chunk at a time, and per chunk
+// frame_encode.cu — the device half of the LZ4 Frame writer (compress_frames_dev in containers.cu, behind
+// b200lz4f_compress_dev and b200lz4f_compress_host_hc): what LZ4FrameOutputStream.writeHeader / writeBlock / writeEndMark
+// write (LZ4FrameOutputStream.java:178-251), for many frames whose bytes are in device memory.  The host only plans (blocks,
+// items, chunks: no payload byte is touched).  The blocks are compressed by the library's batch compressors into bound-sized
+// slots one chunk at a time, and per chunk
 //   frame_size_kernel    the bytes every item takes in its frame (block word, stored or compressed payload, block
 //                        checksum slot; the header on a frame's first item, EndMark and content checksum on its last)
 //   compact_scan_kernel  where every item goes (compact.cu), the running offset carried from chunk to chunk on the device
@@ -18,12 +19,23 @@ __device__ __forceinline__ int frame_header_bytes(int flags) { return 4 + 2 + ((
 __device__ __forceinline__ int frame_tail_bytes(int flags) { return 4 + ((flags & 1) ? 4 : 0); }            // EndMark [checksum]
 __device__ __forceinline__ bool item_first(const FramePlan& p, uint32_t i) { return i == 0 || p.i_frame[i - 1] != p.i_frame[i]; }
 __device__ __forceinline__ bool item_last(const FramePlan& p, uint32_t i) { return i + 1 == p.nitems || p.i_frame[i + 1] != p.i_frame[i]; }
-// stored as is when compression does not shrink the block (LZ4FrameOutputStream.java:215-222), the host writer's rule
+// stored as is when compression does not shrink the block (LZ4FrameOutputStream.java:215-222)
 __device__ __forceinline__ bool block_stored(int32_t clen, int32_t slen) { return clen <= 0 || clen >= slen; }
 
 __device__ __forceinline__ void put_le32(uint8_t* p, uint32_t v)
 {
     p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24);
+}
+
+// The frame descriptor writeHeader puts between the magic and the header checksum byte (LZ4FrameOutputStream.java:178-187):
+// FLG, BD and, with flags bit 2, the 8-byte content size.  Returns the bytes written, 2 or 10.
+__device__ __forceinline__ int frame_descriptor(uint8_t* d, int bsCode, int flags, uint64_t content_size)
+{
+    d[0] = (uint8_t)((1 << 6) | (1 << 5) | ((flags & 2) ? 1 << 4 : 0) | ((flags & 4) ? 1 << 3 : 0) | ((flags & 1) ? 1 << 2 : 0));
+    d[1] = (uint8_t)(bsCode << 4);
+    if (!(flags & 4)) return 2;
+    for (int k = 0; k < 8; k++) d[2 + k] = (uint8_t)(content_size >> (8 * k));
+    return 10;
 }
 
 // XXH32 with seed 0 of fewer than 16 bytes (the frame descriptor): no stripes, the tail and the avalanche of xxhash.c:290-348

@@ -57,18 +57,9 @@ cudaError_t launch_compact(const uint8_t* slots, const uint64_t* slot_off, const
 // NULL: 0).  carry_in and total must be different words.
 cudaError_t launch_scan(const int32_t* lens, uint64_t* out_off, uint64_t* total, const uint64_t* carry_in, size_t n, cudaStream_t st);
 
-// ---- device-resident LZ4 Frame writer (frame_encode.cu, driven by b200lz4f_compress_dev in containers.cu)
-// The frame descriptor LZ4FrameOutputStream.writeHeader puts between the magic and the header checksum byte
-// (LZ4FrameOutputStream.java:178-187): FLG, BD and, with flags bit 2, the 8-byte content size.  flags: bit0 content
-// checksum, bit1 block checksums, bit2 content size.  Returns the bytes written, 2 or 10.  Both frame writers call it.
-__host__ __device__ inline int frame_descriptor(uint8_t* d, int bsCode, int flags, uint64_t content_size)
-{
-    d[0] = (uint8_t)((1 << 6) | (1 << 5) | ((flags & 2) ? 1 << 4 : 0) | ((flags & 4) ? 1 << 3 : 0) | ((flags & 1) ? 1 << 2 : 0));
-    d[1] = (uint8_t)(bsCode << 4);
-    if (!(flags & 4)) return 2;
-    for (int k = 0; k < 8; k++) d[2 + k] = (uint8_t)(content_size >> (8 * k));
-    return 10;
-}
+// ---- LZ4 Frame writer (frame_encode.cu, driven by compress_frames_dev in containers.cu for b200lz4f_compress_dev, and for
+// b200lz4f_compress_host_hc on a device copy of its source).  flags: bit0 content checksum, bit1 block checksums, bit2
+// content size.
 
 // One call's descriptors, all device pointers.  An "item" is one block of a frame, or an empty frame (no block): the frame
 // header rides on a frame's first item, the EndMark and content checksum on its last, so one scan of the item sizes places
@@ -211,11 +202,12 @@ struct Drain {
 // The frame calls' second stream, one per thread and device: the writer's content checksums and the reader's chained content
 // checksums run on it beside the caller's stream, from `fork` on, and every call joins it (`join`) before it returns.
 struct SideStream { cudaStream_t st = nullptr; cudaEvent_t fork = nullptr, join = nullptr; };
-// Grow-or-keep scratch of b200lz4f_compress_dev, one per thread and device (it lives in the thread's context).
+// Grow-or-keep scratch of the frame writer, one per thread and device (it lives in the thread's context).
 struct FrameScratch {
     uint8_t* d_plan = nullptr; size_t plan_cap = 0;        // the call's descriptors (FramePlan)
     uint8_t* h_plan = nullptr; size_t h_plan_cap = 0;      // pinned: their upload, and the results coming back
     uint8_t* d_slots = nullptr; size_t slots_cap = 0;      // one chunk's compressed blocks, bound-sized slots
+    uint8_t* d_stage = nullptr; size_t stage_cap = 0;      // b200lz4f_compress_host_hc: the source at its 16-byte phase, then the frame
 };
 // Grow-or-keep scratch of the frame reader, same lifetime.  d_seg / h_seg serve every step in turn: the device walk, then
 // decode_dev's descriptors and results, then the packing descriptors.
@@ -228,7 +220,7 @@ struct FrameReadScratch {
 };
 // Both select the thread's device, like every entry point.  side (may be NULL): the side stream, created at its first use.
 // idle (may be NULL): a stream of the thread's context that no call keeps busy between calls.
-int get_frame_scratch(FrameScratch** out, SideStream** side);
+int get_frame_scratch(FrameScratch** out, SideStream** side = nullptr, cudaStream_t* idle = nullptr);
 int get_frame_read_scratch(FrameReadScratch** out, SideStream** side = nullptr, cudaStream_t* idle = nullptr);
 
 } // namespace b200

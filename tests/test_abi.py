@@ -53,6 +53,7 @@ def test_no_device_is_loud(b200):
     dst = np.zeros(200, dtype=np.uint8)
     assert lib.b200lz4_compress_default(src.ctypes.data, dst.ctypes.data, 100, 200) == b200._native.E_NODEVICE
     assert "cuda" in b200._native.last_error().lower()
+    assert lib.b200lz4f_compress_host(src.ctypes.data, 0, dst.ctypes.data, 64, 4, 1) == b200._native.E_NODEVICE
     with pytest.raises(b200.B200Error):
         b200.LZ4Factory.b200Instance()
     with pytest.raises(b200.B200Error):

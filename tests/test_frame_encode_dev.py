@@ -1,7 +1,9 @@
-"""b200lz4f_compress_dev: LZ4 frames of device-resident bytes, written on the device.  Every frame must be the host writer's
-(b200lz4f_compress_host_hc) byte for byte at the same source phase, and must be read back by this library's frame reader, the
-restated LZ4FrameInputStream and the reference's LZ4F_decompress.  Runs on the H100, and on the CPU emulator build of the
-library (B200LZ4_TEST_SO=.../libb200lz4_sim.so), where the sizes shrink and torch is not used."""
+"""b200lz4f_compress_dev: LZ4 frames of device-resident bytes, written on the device, and b200lz4f_compress_host_hc, the same
+writer on a device copy of a host source.  Every frame of the fast compressor must be byte for byte the frame assembled here
+by LZ4FrameOutputStream's rules from this library's block compressor at the same source phase (_expected_frame), and every
+frame must be read back by this library's frame reader, the restated LZ4FrameInputStream and the reference's LZ4F_decompress.
+Runs on the H100, and on the CPU emulator build of the library (B200LZ4_TEST_SO=.../libb200lz4_sim.so), where the sizes
+shrink and torch is not used."""
 import os
 import random
 
@@ -83,8 +85,33 @@ def _frames(out, fo, fl):
     return [out[int(o):int(o) + int(n)].tobytes() for o, n in zip(fo, fl)]
 
 
-def _host_frame(b200, data, bs_code, flags, hc=0, phase=0):
-    return b200.compress_frame(_aligned(data, phase), bs_code, bool(flags & 1), bool(flags & 2), bool(flags & 4), hc_level=hc)
+def _expected_frame(b200, port, data, bs_code, flags, phase=0):
+    """the frame LZ4FrameOutputStream writes for `data` (LZ4FrameOutputStream.java:178-251), its blocks compressed by this
+    library's fast block compressor as the frame writer runs it: one batch over the frame's blocks at the source's 16-byte
+    phase, compressBound capacity each, max_src_len 65536 for 64 KiB blocks (GPU streams are not the CPU restatement's)"""
+    flg = 0x60 | (0x10 if flags & 2 else 0) | (0x08 if flags & 4 else 0) | (0x04 if flags & 1 else 0)
+    desc = bytes([flg, bs_code << 4]) + (len(data).to_bytes(8, "little") if flags & 4 else b"")
+    out = bytearray(b"\x04\x22\x4d\x18" + desc + bytes([(port.xxh32(desc, 0) >> 8) & 0xFF]))
+    bs = 1 << (8 + 2 * bs_code)
+    if data:
+        offs = np.arange(0, len(data), bs, dtype=np.uint64)
+        lens = np.minimum(bs, len(data) - offs).astype(np.int32)
+        cap = lens + lens // 255 + 16
+        slot = (cap.astype(np.uint64) + 15) // 16 * 16
+        coff = np.cumsum(slot) - slot
+        comp = np.zeros(int(slot.sum()), dtype=np.uint8)
+        clen = b200.batch.compress_fast_batch_host(_aligned(data, phase), offs, lens, comp, coff, cap,
+                                                   max_src_len=65536 if bs <= 65536 else 0)
+        for o, n, co, c in zip(offs.tolist(), lens.tolist(), coff.tolist(), clen.tolist()):
+            stored = c <= 0 or c >= n                                   # (:215-222)
+            payload = data[o:o + n] if stored else comp[co:co + c].tobytes()
+            out += (len(payload) | (0x80000000 if stored else 0)).to_bytes(4, "little") + payload
+            if flags & 2:
+                out += port.xxh32(payload, 0).to_bytes(4, "little")
+    out += bytes(4)                                                     # EndMark
+    if flags & 1:
+        out += port.xxh32(data, 0).to_bytes(4, "little")
+    return bytes(out)
 
 
 def _reference():
@@ -115,8 +142,8 @@ def _mixed(port):
 
 
 def test_frames_equal_the_host_writer_and_every_reader_reads_them(b200, port):
-    """every bsCode 4..7 and flags 0..7 over one mixed call at 64-byte-aligned device offsets: each frame is the host
-    writer's, frame_off is contiguous from 0, the return value is the sum of frame_len, and the frames decode with this
+    """every bsCode 4..7 and flags 0..7 over one mixed call at 64-byte-aligned device offsets: each frame is the expected
+    one, frame_off is contiguous from 0, the return value is the sum of frame_len, and the frames decode with this
     library's reader (all of them at once), the restated LZ4FrameInputStream and the reference's LZ4F_decompress"""
     L, M, ref = b200._native.lib(), _DevMem(), _reference()
     datas = _mixed(port)
@@ -132,13 +159,13 @@ def test_frames_equal_the_host_writer_and_every_reader_reads_them(b200, port):
         out = M.down(d_dst)
         frames = _frames(out, fo, fl_)
         for k, (f, d) in enumerate(zip(frames, datas)):
-            assert f == _host_frame(b200, d, bs, fl), (bs, fl, k, len(d))
+            assert f == _expected_frame(b200, port, d, bs, fl), (bs, fl, k, len(d))
         _check_readers(b200, port, ref, frames, datas, out[:rc].tobytes())
 
 
 def test_unaligned_sources_give_valid_frames(b200, port):
     """sources at offsets 1, 2, 3 and 7 (mod 16): the compressor may parse differently there (DESIGN.md §4, source
-    alignment), so the frames need not be the host writer's, but they are valid and decode to their input"""
+    alignment), so the frames need not be those of 16-byte-aligned sources, but they are valid and decode to their input"""
     L, M, ref = b200._native.lib(), _DevMem(), _reference()
     data = port.datagen(200000 if SIM else 2000000, 0.5, 0.0, 4).tobytes()
     datas = [data[:n] for n in (70000, 1, 0, 150000 if SIM else 1500000, 65536)]
@@ -153,7 +180,7 @@ def test_unaligned_sources_give_valid_frames(b200, port):
 
 def test_high_compressor_frames(b200, port):
     """hc_level 3, 9, 12: readable by every reader and no larger than the fast compressor's frames on compressible data
-    (not byte-identical to the host writer: the HC kernel's ring insert order comes from atomicAdd)"""
+    (not byte-identical from call to call: the HC kernel's ring insert order comes from atomicAdd)"""
     L, M, ref = b200._native.lib(), _DevMem(), _reference()
     datas = [port.datagen(n, 0.5, 0.0, 5 + n % 7).tobytes() for n in ((70000, 1) if SIM else (300000, 65537, 1, 0, 1500000))]
     src, offs, lens = _lay_out(datas)
@@ -168,7 +195,7 @@ def test_high_compressor_frames(b200, port):
 
 
 def test_calls_that_span_several_chunks(b200, port):
-    """a call cut into several internal chunks (CHUNK_SPAN, B200LZ4_CHUNK_MB) is the host writer's, frame by frame: the
+    """a call cut into several internal chunks (CHUNK_SPAN, B200LZ4_CHUNK_MB) is the expected one, frame by frame: the
     running offset is carried from chunk to chunk on the device"""
     L, M = b200._native.lib(), _DevMem()
     total = (2 << 20) if SIM else (600 << 20)
@@ -182,7 +209,21 @@ def test_calls_that_span_several_chunks(b200, port):
         assert rc == int(fl_.sum()), (bs, fl)
         out = M.down(d_dst)
         for k, (f, d) in enumerate(zip(_frames(out, fo, fl_), datas)):
-            assert f == _host_frame(b200, d, bs, fl), (bs, fl, k)
+            assert f == _expected_frame(b200, port, d, bs, fl), (bs, fl, k)
+
+
+def test_host_writer_keeps_the_source_phase(b200, port):
+    """b200lz4f_compress_host_hc (compress_frame) stages the source at its own 16-byte phase before the device writer runs,
+    so its frame is the expected one at that phase; the phases chosen give different frames for the longest source"""
+    data = port.datagen(200000, 0.5, 0.0, 13).tobytes()
+    sizes = (0, 1, 65536, 65537) if SIM else (0, 1, 100, 65536, 65537, 200000)
+    for n in sizes:
+        for fl in (0, 7):
+            want = {p: _expected_frame(b200, port, data[:n], 4, fl, p) for p in (0, 1, 3, 8)}
+            for p, w in want.items():
+                got = b200.compress_frame(_aligned(data[:n], p), 4, bool(fl & 1), bool(fl & 2), bool(fl & 4))
+                assert got == w, (n, fl, p)
+    assert len(set(want.values())) > 1
 
 
 @pytest.mark.skipif(SIM, reason="torch streams: GPU only")
@@ -205,7 +246,7 @@ def test_ordered_after_the_stream_and_nothing_written_past_the_frames(b200, port
     out = M.down(d_dst)
     assert rc == int(fl_.sum())
     for f, d in zip(_frames(out, fo, fl_), datas):
-        assert f == _host_frame(b200, d, 4, 7)
+        assert f == _expected_frame(b200, port, d, 4, 7)
     assert (out[rc:] == 0xAA).all()
 
 

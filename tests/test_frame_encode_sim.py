@@ -20,4 +20,4 @@ def test_device_frame_writer_on_the_emulator_library(sim_library):
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(HERE, "test_frame_encode_dev.py"), "-m", "gpu", "-q", "-x",
                         "-p", "no:cacheprovider", "-W", "ignore::DeprecationWarning"],
                        env=env, cwd=os.path.dirname(HERE), capture_output=True, text=True)
-    assert r.returncode == 0 and "6 passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+    assert r.returncode == 0 and "7 passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
