@@ -288,6 +288,34 @@ int64_t b200lz4block_compress_host_hc(const uint8_t* src, size_t srcSize, uint8_
  * reads concatenated streams to the end of src. */
 int64_t b200lz4block_decompress_host(const uint8_t* src, size_t srcSize, uint8_t* dst, size_t dstCapacity,
                                      int stopOnEmptyBlock, size_t* srcConsumed);
+
+/* Device-resident LZ4Block writer (LZ4BlockOutputStream.java:203-266) for ns independent streams.  Stream s is src_len[s]
+ * bytes at d_src + src_off[s] (HOST arrays; the bytes are in device memory of the current device); the streams are written
+ * back to back into d_dst, stream_off / stream_len (host, may be NULL) say where.  Each stream is byte for byte what
+ * b200lz4block_compress_host_hc writes for the same bytes at the same 16-byte phase (that call is this writer run on a device
+ * copy of its source).  blockSize 64..32 MiB (any value; the token's level nibble comes from it), hc_level 0 = the fast
+ * compressor, 1..17 = LZ4_compress_HC at that level.  Returns the total bytes written, or: -9 dst_capacity < sum of
+ * b200lz4block_compress_bound(src_len[s], blockSize); B200LZ4_E_ARG, _CUDA, _NODEVICE.  Argument and size errors are found
+ * before anything is launched or written.  Ordered after the work already queued on `stream`; returns when the streams are
+ * in d_dst.  Grow-or-keep scratch of the thread's context: the frame writer's. */
+int64_t b200lz4block_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                  uint8_t* d_dst, size_t dst_capacity, uint64_t* stream_off, uint64_t* stream_len,
+                                  int blockSize, int hc_level, void* stream);
+
+/* Device-resident LZ4Block reader (LZ4BlockInputStream.java:191-264) for ns independent streams, each read as its own
+ * LZ4BlockInputStream(in, stopOnEmptyBlock).  Stream s: src_len[s] bytes at d_src + src_off[s], decoded to d_dst + dst_off[s]
+ * with room dst_cap[s] (all offset / length arrays HOST, the bytes device memory of the current device).  result[s] is what
+ * b200lz4block_decompress_host returns for the same bytes and capacity, src_consumed[s] (may be NULL) what it reports in
+ * *srcConsumed (0 when result[s] < 0).  content_len[s] (may be NULL): what the stream decodes to when room is not the limit;
+ * it equals result[s] when result[s] >= 0, and when result[s] == -9 a second call with dst_cap[s] = content_len[s] does not
+ * return -9.  On success nothing in d_dst outside [dst_off[s], dst_off[s] + result[s]) is written for stream s; on an error
+ * [dst_off[s], dst_off[s] + dst_cap[s]) holds unspecified bytes and nothing outside it is written.  No payload byte crosses to
+ * the host: per stream its arguments go up and its results come back, and two block counts in between.  Returns 0 or
+ * B200LZ4_E_*.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep
+ * scratch of the thread's context: the frame reader's. */
+int     b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                    uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int stopOnEmptyBlock,
+                                    int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream);
 int     b200lz4_compress_with_length(const char* src, char* dst, int srcSize, int dstCapacity);
 int     b200lz4_decompressed_length(const char* src);
 int     b200lz4_decompress_with_length(const char* src, int srcAvail, char* dst, int dstCapacity);

@@ -4,13 +4,16 @@
 //   * "LZ4Block" container — LZ4BlockOutputStream.flushBufferedData/finish (:203-266) and
 //                            LZ4BlockInputStream.refill (LZ4BlockInputStream.java:191-264)
 //   * length-prefixed block — LZ4CompressorWithLength / LZ4DecompressorWithLength
-// The reference does these one block per native call.  Here the frame is written on the device (frame_encode.cu), and the
-// LZ4Block container's host code only lays out headers while the payload work (block compression / decompression, every
-// XXH32) goes through the batch entry points, i.e. the CUDA kernels.  No hashing or codec arithmetic runs on the host.
+// The reference does these one block per native call.  Here both containers are written on the device, by one loop
+// (compress_blocks_dev) with the kernels of frame_encode.cu and lz4block.cu; the host writers run it on a device copy of their
+// source.  The LZ4Block reader walks the headers with walk_lz4block (kernels.h): on the host for host buffers, whose payload
+// work (block decompression, every XXH32) goes through the batch entry points, and on the device for streams in device
+// memory (lz4block.cu).  No hashing or codec arithmetic runs on the host.
 #include "../../include/b200lz4.h"
 #include "kernels.h"
-#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device frame writer's kernels come with it
+#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device writers' and reader's kernels come with it
 #include "frame_encode.cu"
+#include "lz4block.cu"
 #endif
 #include <cstdlib>
 #include <cstring>
@@ -19,23 +22,7 @@
 static inline void put32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
 static inline uint32_t get32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
 
-// The LZ4Block writer's compressor argument (LZ4BlockOutputStream takes any LZ4Compressor): hc_level 0 = the fast
-// compressor, packed output; 1..17 = LZ4_compress_HC at that level into bound-sized slots.  coff/clen as *_compact_host.
-static int compress_blocks(const uint8_t* src, const uint64_t* soff, const int32_t* slen, uint8_t* tmp, size_t tmp_cap,
-                           uint64_t* coff, int32_t* clen, size_t nb, int max_src_len, int hc_level)
-{
-    if (hc_level <= 0) {
-        uint64_t total = 0;
-        return b200lz4_compress_fast_compact_host(src, soff, slen, tmp, tmp_cap, coff, clen, nb, max_src_len, &total);
-    }
-    std::vector<int32_t> ccap(nb);
-    uint64_t acc = 0;
-    for (size_t i = 0; i < nb; i++) { coff[i] = acc; ccap[i] = (int32_t)b200::compress_bound((uint64_t)slen[i]); acc += b200::aligned_compress_bound((uint64_t)slen[i]); }
-    if (acc > tmp_cap) return B200LZ4_E_ARG;
-    return b200lz4_compress_hc_batch_host(src, soff, slen, tmp, coff, ccap.data(), clen, nb, hc_level);
-}
-
-// ---------------------------------------------------------------- LZ4 Frame writer (frame_encode.cu)
+// ---------------------------------------------------------------- LZ4 Frame and LZ4Block writers (frame_encode.cu, lz4block.cu)
 namespace b200 {
 
 // Where the FramePlan arrays of a call with nb blocks, ni items and nf frames lie in one blob, the same on the host and the
@@ -57,21 +44,26 @@ struct FramePlanLayout {
 
 struct FrameChunk { size_t i0, i1, b0, b1; };                       // items [i0, i1), their blocks [b0, b1)
 
-static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
-                                   uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
-                                   int bsCode, int flags, int hc_level, cudaStream_t st)
+// The two containers written on the device.  An LZ4Block "frame" is one stream: blocks of blockSize bytes, the end block on
+// its last item, checksums of the original blocks.
+enum class Container { Frame, LZ4Block };
+
+// Both writers: arguments and sizes (nothing is launched or written before these pass), the plan, the chunk loop and the
+// results.  Only the item sizes, the emit, the checksums and the seal differ by container.  bs: bytes per block; code:
+// the frame's bsCode or the LZ4Block token's level nibble; flags: the frame's (0 for LZ4Block).
+static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                   size_t nf, uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
+                                   uint64_t bs, int code, int flags, int hc_level, cudaStream_t st)
 {
-    // ---- arguments and sizes: nothing is launched or written before these pass
-    if (bsCode < 4 || bsCode > 7) return fail_arg("bsCode must be 4..7");
+    const bool frame = kind == Container::Frame;
     if (nf == 0) return 0;
     if (!src_off || !src_len || !d_dst) return fail_arg("null pointer");
-    const uint64_t bs = 1ull << (8 + 2 * bsCode);
     uint64_t need = 0, nb = 0, ni = 0, bytes = 0;
     bool too_long = false;
     for (size_t f = 0; f < nf; f++) {
         const uint64_t n = src_len[f];
         if (n > (1ull << 47)) return fail_arg("src_len");
-        need += b200lz4f_compress_bound(n, bsCode);
+        need += frame ? b200lz4f_compress_bound(n, code) : b200lz4block_compress_bound(n, (int)bs);
         nb += (n + bs - 1) / bs; ni += n ? (n + bs - 1) / bs : 1; bytes += n;
         if ((flags & 1) && n > 0x7FFFFFFFull) too_long = true;
     }
@@ -122,18 +114,25 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
                        (uint64_t*)(D + L.b_poff), (int32_t*)(D + L.b_plen), (const uint32_t*)(D + L.b_sum),
                        (const uint32_t*)(D + L.i_frame), (const int32_t*)(D + L.i_block), (int32_t*)(D + L.i_size), (uint64_t*)(D + L.i_off),
                        (const uint64_t*)(D + L.f_len), (const uint32_t*)(D + L.f_sum), (uint64_t*)(D + L.f_off), (uint64_t*)(D + L.f_end),
-                       (uint32_t)ni, bsCode, flags };
+                       (uint32_t)ni, frame ? code : 0, flags, frame ? 0 : code };
     uint64_t* carry = (uint64_t*)(D + L.carry);
 
     // ---- launches, all ordered after what `st` already holds
     Drain drain{ st, side->st };
     auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
-    if (flags & 1) {                // content checksums: the sources only, so from the start, beside everything else
+    // checksums of the sources alone, so from the start, beside everything else: the frame's content checksums, or the
+    // LZ4Block checksums of the original blocks
+    const bool early_sums = frame ? (flags & 1) != 0 : nb > 0;
+    if (early_sums) {
         CK(cudaEventRecord(side->fork, st));
         CK(cudaStreamWaitEvent(side->st, side->fork, 0));
-        CK(counted(launch_xxh32_long(d_src, (const uint64_t*)(D + L.f_soff), (const int32_t*)(D + L.f_len32), 0,
-                                     (uint32_t*)(D + L.f_sum), nf, side->st)));
+        if (frame)
+            CK(counted(launch_xxh32_long(d_src, (const uint64_t*)(D + L.f_soff), (const int32_t*)(D + L.f_len32), 0,
+                                         (uint32_t*)(D + L.f_sum), nf, side->st)));
+        else
+            CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+                d_src, P.b_soff, P.b_slen, LZ4BLOCK_SEED, (uint32_t*)P.b_sum, (size_t)nb, side->st)));
         CK(cudaEventRecord(side->join, side->st));
     }
     for (size_t k = 0; k < chunks.size(); k++) {
@@ -144,16 +143,16 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
             CK(counted(hc_level > 0 ? launch_compress_hc(a, hc_level, st) : launch_compress_fast(a, bs <= 65536 ? 65536 : 0, st)));
         }
         const uint32_t i0 = (uint32_t)c.i0, n = (uint32_t)(c.i1 - c.i0);
-        CK(counted(launch_frame_sizes(P, i0, n, st)));
+        CK(counted(frame ? launch_frame_sizes(P, i0, n, st) : launch_lz4block_sizes(P, i0, n, st)));
         CK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
-        CK(counted(launch_frame_emit(P, i0, n, st)));
+        CK(counted(frame ? launch_frame_emit(P, i0, n, st) : launch_lz4block_emit(P, i0, n, st)));
     }
     if ((flags & 2) && nb) {        // block checksums over the payloads as written; the source average bounds the payloads'
         CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
             d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
     }
-    if (flags & 1) CK(cudaStreamWaitEvent(st, side->join, 0));
-    CK(counted(launch_frame_seal(P, st)));
+    if (early_sums) CK(cudaStreamWaitEvent(st, side->join, 0));
+    CK(counted(frame ? launch_frame_seal(P, st) : launch_lz4block_seal(P, st)));
     CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     drain.done = true;
@@ -163,6 +162,173 @@ static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off
     }
     return (int64_t)h64(L.carry)[chunks.size() & 1];
 }
+
+static int64_t compress_frames_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
+                                   uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
+                                   int bsCode, int flags, int hc_level, cudaStream_t st)
+{
+    if (bsCode < 4 || bsCode > 7) return fail_arg("bsCode must be 4..7");
+    return compress_blocks_dev(Container::Frame, d_src, src_off, src_len, nf, d_dst, dst_capacity, frame_off, frame_len,
+                               1ull << (8 + 2 * bsCode), bsCode, flags, hc_level, st);
+}
+
+static int lz4block_level(int blockSize)                                        // LZ4BlockOutputStream.java:58-70
+{
+    int lvl = 0; while ((1 << lvl) < blockSize) lvl++;                           // 32 - numberOfLeadingZeros(blockSize - 1)
+    lvl -= 10; return lvl < 0 ? 0 : lvl;
+}
+
+static int64_t compress_lz4block_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                     uint8_t* d_dst, size_t dst_capacity, uint64_t* stream_off, uint64_t* stream_len,
+                                     int blockSize, int hc_level, cudaStream_t st)
+{
+    if (blockSize < 64 || blockSize > (1 << 25)) return fail_arg("blockSize must be 64..32 MiB");
+    return compress_blocks_dev(Container::LZ4Block, d_src, src_off, src_len, ns, d_dst, dst_capacity, stream_off, stream_len,
+                               (uint64_t)blockSize, lz4block_level(blockSize), 0, hc_level, st);
+}
+
+// A device writer, write(d_src, src_off, src_len, d_dst, capacity, st) for one source, run on a copy of src in the thread's
+// staging buffer: the source at its own 16-byte phase (the fast compressor's chunks, and so its streams, follow the source's
+// alignment), the container behind it.  bound: the container's size bound, checked against cap by the caller.
+template <class Write>
+static int64_t write_staged(const uint8_t* src, size_t n, uint8_t* dst, size_t bound, Write write)
+{
+    FrameScratch* s; cudaStream_t st;
+    int rc = get_frame_scratch(&s, nullptr, &st); if (rc) return rc;
+    const uint64_t phase = (uintptr_t)src & 15, len = n, at = (phase + n + 15) & ~uint64_t(15);
+    rc = reserve_device(s->d_stage, s->stage_cap, at + bound); if (rc) return rc;
+    Drain drain{ st };
+    CK(cudaMemcpyAsync(s->d_stage + phase, src, n, cudaMemcpyHostToDevice, st));
+    const int64_t w = write(s->d_stage, &phase, &len, s->d_stage + at, bound, st);
+    if (w < 0) return w;
+    CK(cudaMemcpyAsync(dst, s->d_stage + at, (size_t)w, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    return w;
+}
+
+// ---------------------------------------------------------------- LZ4Block reader, streams in device memory (lz4block.cu)
+// Where one call's per-stream arrays lie in the reader scratch's d_seg / h_seg: the inputs go up, the two block counts come
+// back after the counting walk, the results (result, consumed, content) at the end.
+struct Lz4BlockStreamLayout {
+    size_t s_off, s_len, d_off, d_cap, n_comp, n_raw, tail, ip, p_comp, p_raw, totals, result, consumed, content, bytes = 0;
+    explicit Lz4BlockStreamLayout(size_t ns)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        s_off = take(8 * ns); s_len = take(8 * ns); d_off = take(8 * ns); d_cap = take(8 * ns);
+        n_comp = take(4 * ns); n_raw = take(4 * ns); tail = take(4 * ns); ip = take(8 * ns); p_comp = take(8 * ns); p_raw = take(8 * ns);
+        totals = take(16);
+        result = take(8 * ns); consumed = take(8 * ns); content = take(8 * ns);
+    }
+};
+// ... and the records of nc compressed and nr stored blocks in d_recs; they never leave the device
+struct Lz4BlockRecLayout {
+    size_t c_soff, c_doff, c_clen, c_olen, c_res, r_soff, r_doff, r_len, b_doff, b_len, b_comp, b_want, b_sum, bytes = 0;
+    Lz4BlockRecLayout(size_t nc, size_t nr)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        const size_t nb = nc + nr;
+        c_soff = take(8 * nc); c_doff = take(8 * nc); c_clen = take(4 * nc); c_olen = take(4 * nc); c_res = take(4 * nc);
+        r_soff = take(8 * nr); r_doff = take(8 * nr); r_len = take(4 * nr);
+        b_doff = take(8 * nb); b_len = take(4 * nb); b_comp = take(4 * nb); b_want = take(4 * nb); b_sum = take(4 * nb);
+    }
+};
+
+// Counting walk, two scans of the counts (only their totals come to the host: the records' room), recording walk, then
+// the blocks decode straight into d_dst, their checksums, and one verdict per stream.  The launches do not depend on the
+// number of streams or blocks.
+static int lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                   uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, bool stop,
+                                   int64_t* result, uint64_t* src_consumed, uint64_t* content_len, cudaStream_t st)
+{
+    if (ns == 0) return 0;
+    if (!src_off || !src_len || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
+    if (ns > 0x7FFFFFFFull) return fail_arg("too many streams in one call");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    if (bytes / LZ4BLOCK_HEADER > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
+    FrameReadScratch* s;
+    int rc = get_frame_read_scratch(&s);
+    const Lz4BlockStreamLayout L(ns);
+    if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
+    if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
+    if (rc) return rc;
+    uint8_t *D = s->d_seg, *H = s->h_seg;
+    memcpy(H + L.s_off, src_off, 8 * ns); memcpy(H + L.s_len, src_len, 8 * ns);
+    memcpy(H + L.d_off, dst_off, 8 * ns); memcpy(H + L.d_cap, dst_cap, 8 * ns);
+    Lz4BlockRead r{};
+    r.src = d_src;
+    r.s_off = (const uint64_t*)(D + L.s_off); r.s_len = (const uint64_t*)(D + L.s_len);
+    r.d_off = (const uint64_t*)(D + L.d_off); r.d_cap = (const uint64_t*)(D + L.d_cap);
+    r.n_comp = (int32_t*)(D + L.n_comp); r.n_raw = (int32_t*)(D + L.n_raw); r.tail = (int32_t*)(D + L.tail);
+    r.ip = (uint64_t*)(D + L.ip); r.content = (uint64_t*)(D + L.content);
+    r.p_comp = (const uint64_t*)(D + L.p_comp); r.p_raw = (const uint64_t*)(D + L.p_raw);
+    r.result = (int64_t*)(D + L.result); r.consumed = (uint64_t*)(D + L.consumed);
+    r.ns = (uint32_t)ns; r.stop = stop;
+    uint64_t* totals = (uint64_t*)(D + L.totals);
+
+    Drain drain{ st };
+    CK(cudaMemcpyAsync(D, H, L.n_comp, cudaMemcpyHostToDevice, st));
+    g_launch_count.fetch_add(3, std::memory_order_relaxed);
+    CK(launch_lz4block_walk(r, false, st));
+    CK(launch_scan(r.n_comp, (uint64_t*)r.p_comp, totals, nullptr, ns, st));
+    CK(launch_scan(r.n_raw, (uint64_t*)r.p_raw, totals + 1, nullptr, ns, st));
+    CK(cudaMemcpyAsync(H + L.totals, totals, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint64_t nc = ((const uint64_t*)(H + L.totals))[0], nr = ((const uint64_t*)(H + L.totals))[1], nb = nc + nr;
+    const Lz4BlockRecLayout R(nc, nr);
+    rc = reserve_device(s->d_recs, s->recs_cap, R.bytes + 16); if (rc) return rc;
+    uint8_t* B = s->d_recs;
+    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
+    r.c_clen = (int32_t*)(B + R.c_clen); r.c_olen = (int32_t*)(B + R.c_olen); r.c_res = (int32_t*)(B + R.c_res);
+    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
+    r.b_doff = (uint64_t*)(B + R.b_doff); r.b_len = (int32_t*)(B + R.b_len); r.b_comp = (int32_t*)(B + R.b_comp);
+    r.b_want = (uint32_t*)(B + R.b_want); r.b_sum = (uint32_t*)(B + R.b_sum);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
+    CK(launch_lz4block_walk(r, true, st));
+    if (nr) {
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        CK(launch_gather(d_src, r.r_soff, r.r_len, d_dst, r.r_doff, (size_t)nr, st));
+    }
+    if (nc) {                       // as the host reader: src_avail = the compressed length, dst_len = the original length
+        const BatchArgs a{ d_src, r.c_soff, r.c_clen, d_dst, r.c_doff, r.c_olen, r.c_res, (size_t)nc };
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        CK(launch_decompress_fast(a, st));
+    }
+    if (nb) {                       // the decoded bytes are at most the room given, and at most 255 per source byte
+        const uint64_t decoded = room < bytes * 255 ? room : bytes * 255;
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        CK((decoded / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_dst, r.b_doff, r.b_len, LZ4BLOCK_SEED, r.b_sum, (size_t)nb, st));
+    }
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
+    CK(launch_lz4block_verdict(r, st));
+    CK(cudaMemcpyAsync(H + L.result, D + L.result, L.bytes - L.result, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    memcpy(result, H + L.result, 8 * ns);
+    if (src_consumed) memcpy(src_consumed, H + L.consumed, 8 * ns);
+    if (content_len) memcpy(content_len, H + L.content, 8 * ns);
+    return 0;
+}
+
+// The host reader's sink of walk_lz4block: the stored blocks that fit are copied at once, the compressed ones and every
+// checksum go to the batch calls afterwards.
+struct Lz4BlockHostSink {
+    const uint8_t* src; uint8_t* dst; Lz4BlockRoom room;
+    std::vector<uint64_t> soff, doff, hoff; std::vector<int32_t> savail, dlen, hlen; std::vector<uint32_t> want;
+    void block(uint64_t at, bool raw, int32_t clen, int32_t olen, uint32_t check)
+    {
+        const uint64_t op = room.used;
+        if (!room.take(olen)) return;
+        if (raw) memcpy(dst + op, src + at, (size_t)olen);
+        else { soff.push_back(at); savail.push_back(clen); doff.push_back(op); dlen.push_back(olen); }
+        hoff.push_back(op); hlen.push_back(olen); want.push_back(check);
+    }
+};
 
 } // namespace b200
 
@@ -183,83 +349,46 @@ int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, con
                                      hc_level, (cudaStream_t)stream);
 }
 
-// The device writer on a copy of src in the thread's staging buffer: the source at its own 16-byte phase (the fast
-// compressor's chunks, and so its streams, follow the source's alignment), the frame behind it.
+// The device writer on a staged copy of src (write_staged)
 int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags, int hc_level)
 {
     if (bsCode < 4 || bsCode > 7) return b200::fail_arg("bsCode must be 4..7");
     const size_t bound = b200lz4f_compress_bound(n, bsCode);
     if (cap < bound) return -9;
-    b200::FrameScratch* s; cudaStream_t st;
-    int rc = b200::get_frame_scratch(&s, nullptr, &st); if (rc) return rc;
-    const uint64_t phase = (uintptr_t)src & 15, len = n, at = (phase + n + 15) & ~uint64_t(15);
-    rc = b200::reserve_device(s->d_stage, s->stage_cap, at + bound); if (rc) return rc;
-    b200::Drain drain{ st };
-    CK(cudaMemcpyAsync(s->d_stage + phase, src, n, cudaMemcpyHostToDevice, st));
-    const int64_t w = b200::compress_frames_dev(s->d_stage, &phase, &len, 1, s->d_stage + at, bound, nullptr, nullptr, bsCode,
-                                                flags, hc_level, st);
-    if (w < 0) return w;
-    CK(cudaMemcpyAsync(dst, s->d_stage + at, (size_t)w, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    drain.done = true;
-    return w;
+    return b200::write_staged(src, n, dst, bound, [&](const uint8_t* d_src, const uint64_t* off, const uint64_t* len, uint8_t* d_dst,
+                                                      size_t room, cudaStream_t st) {
+        return b200::compress_frames_dev(d_src, off, len, 1, d_dst, room, nullptr, nullptr, bsCode, flags, hc_level, st);
+    });
 }
 int64_t b200lz4f_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags)
 { return b200lz4f_compress_host_hc(src, n, dst, cap, bsCode, flags, 0); }
 
 // ---------------------------------------------------------------- "LZ4Block" container
-static const uint8_t LZ4BLOCK_MAGIC[8] = { 'L', 'Z', '4', 'B', 'l', 'o', 'c', 'k' };
-enum { LZ4BLOCK_HEADER = 8 + 1 + 4 + 4 + 4, METHOD_RAW = 0x10, METHOD_LZ4 = 0x20 };
-static const uint32_t LZ4BLOCK_SEED = 0x9747b28cu;                               // LZ4BlockOutputStream.java:56
-
-static int lz4block_level(int blockSize)                                        // LZ4BlockOutputStream.java:58-70
-{
-    int lvl = 0; while ((1 << lvl) < blockSize) lvl++;                           // 32 - numberOfLeadingZeros(blockSize - 1)
-    lvl -= 10; return lvl < 0 ? 0 : lvl;
-}
-
 size_t b200lz4block_compress_bound(size_t n, int blockSize)
 {
     if (blockSize < 64 || blockSize > (1 << 25)) return 0;
     const size_t nb = (n + blockSize - 1) / blockSize;
-    return (nb + 1) * LZ4BLOCK_HEADER + n + nb * 16 + n / 255;
+    return (nb + 1) * b200::LZ4BLOCK_HEADER + n + nb * 16 + n / 255;
 }
 
+int64_t b200lz4block_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                  uint8_t* d_dst, size_t dst_capacity, uint64_t* stream_off, uint64_t* stream_len,
+                                  int blockSize, int hc_level, void* stream)
+{
+    return b200::compress_lz4block_dev(d_src, src_off, src_len, ns, d_dst, dst_capacity, stream_off, stream_len, blockSize,
+                                       hc_level, (cudaStream_t)stream);
+}
+
+// The device writer on a staged copy of src (write_staged)
 int64_t b200lz4block_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int blockSize, int hc_level)
 {
-    if (blockSize < 64 || blockSize > (1 << 25)) return B200LZ4_E_ARG;
-    if (cap < b200lz4block_compress_bound(n, blockSize)) return -9;
-    const int level = lz4block_level(blockSize);
-    const size_t bs = (size_t)blockSize, nb = (n + bs - 1) / bs;
-    size_t o = 0;
-    if (nb) {
-        std::vector<uint64_t> soff(nb), coff(nb);
-        std::vector<int32_t> slen(nb), clen(nb);
-        std::vector<uint32_t> sums(nb);
-        for (size_t i = 0; i < nb; i++) { soff[i] = i * bs; slen[i] = (int32_t)((n - i * bs) < bs ? (n - i * bs) : bs); }
-        size_t tmp_cap = 0; for (size_t i = 0; i < nb; i++) tmp_cap += (size_t)slen[i] + slen[i] / 255 + 32;
-        uint8_t* tmp = (uint8_t*)malloc(tmp_cap ? tmp_cap : 1);
-        if (!tmp) return B200LZ4_E_ARG;
-        int rc = compress_blocks(src, soff.data(), slen.data(), tmp, tmp_cap, coff.data(), clen.data(), nb, bs <= 65536 ? 65536 : 0, hc_level);
-        if (!rc) rc = b200xxh32_batch_host(src, soff.data(), slen.data(), LZ4BLOCK_SEED, sums.data(), nb);   // checksum of the ORIGINAL bytes
-        if (rc) { free(tmp); return rc; }
-        for (size_t i = 0; i < nb; i++) {                                        // flushBufferedData (:203-227)
-            const bool raw = clen[i] <= 0 || clen[i] >= slen[i];
-            const uint32_t sz = raw ? (uint32_t)slen[i] : (uint32_t)clen[i];
-            memcpy(dst + o, LZ4BLOCK_MAGIC, 8);
-            dst[o + 8] = (uint8_t)((raw ? METHOD_RAW : METHOD_LZ4) | level);
-            put32(dst + o + 9, sz); put32(dst + o + 13, (uint32_t)slen[i]);
-            put32(dst + o + 17, sums[i] & 0x0FFFFFFFu);                          // Checksum view keeps 28 bits (StreamingXXHash32.java:106)
-            memcpy(dst + o + LZ4BLOCK_HEADER, raw ? src + soff[i] : tmp + coff[i], sz);
-            o += LZ4BLOCK_HEADER + sz;
-        }
-        free(tmp);
-    }
-    memcpy(dst + o, LZ4BLOCK_MAGIC, 8);                                          // finish(): empty block (:255-266)
-    dst[o + 8] = (uint8_t)(METHOD_RAW | level);
-    put32(dst + o + 9, 0); put32(dst + o + 13, 0); put32(dst + o + 17, 0);
-    o += LZ4BLOCK_HEADER;
-    return (int64_t)o;
+    if (blockSize < 64 || blockSize > (1 << 25)) return b200::fail_arg("blockSize must be 64..32 MiB");
+    const size_t bound = b200lz4block_compress_bound(n, blockSize);
+    if (cap < bound) return -9;
+    return b200::write_staged(src, n, dst, bound, [&](const uint8_t* d_src, const uint64_t* off, const uint64_t* len, uint8_t* d_dst,
+                                                      size_t room, cudaStream_t st) {
+        return b200::compress_lz4block_dev(d_src, off, len, 1, d_dst, room, nullptr, nullptr, blockSize, hc_level, st);
+    });
 }
 int64_t b200lz4block_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int blockSize)
 { return b200lz4block_compress_host_hc(src, n, dst, cap, blockSize, 0); }
@@ -271,45 +400,36 @@ int64_t b200lz4block_compress_host(const uint8_t* src, size_t n, uint8_t* dst, s
 // Returns decoded bytes; -1 premature end, -2 "Stream is corrupted", -9 dst too small.
 int64_t b200lz4block_decompress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int stopOnEmptyBlock, size_t* srcConsumed)
 {
-    std::vector<uint64_t> soff, doff; std::vector<int32_t> savail, dlen, csz; std::vector<uint32_t> want;
-    std::vector<uint64_t> hoff; std::vector<int32_t> hlen;
-    size_t ip = 0, op = 0;
-    int64_t tail = 0;                    // what is wrong with the container itself, behind the blocks collected so far: the reader
-                                         // would have decoded and checked THOSE first, so their verdict comes first
-    for (;;) {                                                                   // refill (:191-264)
-        if (n - ip < LZ4BLOCK_HEADER) { if (stopOnEmptyBlock) tail = -1; else ip = n; break; }
-        if (memcmp(src + ip, LZ4BLOCK_MAGIC, 8) != 0) { tail = -2; break; }
-        const int token = src[ip + 8], method = token & 0xF0, level = 10 + (token & 0x0F);
-        if (method != METHOD_RAW && method != METHOD_LZ4) { tail = -2; break; }
-        const int32_t clen = (int32_t)get32(src + ip + 9), olen = (int32_t)get32(src + ip + 13);
-        const uint32_t check = get32(src + ip + 17);
-        if (olen > (1 << level) || olen < 0 || clen < 0 || (olen == 0 && clen != 0) || (olen != 0 && clen == 0) ||
-            (method == METHOD_RAW && olen != clen)) { tail = -2; break; }
-        ip += LZ4BLOCK_HEADER;
-        if (olen == 0) { if (check != 0) { tail = -2; break; } if (stopOnEmptyBlock) break; continue; }   // empty block (:225-233)
-        if (n - ip < (size_t)clen) { tail = -1; break; }
-        if (cap - op < (size_t)olen) { tail = -9; break; }
-        if (method == METHOD_RAW) memcpy(dst + op, src + ip, (size_t)olen);
-        else { soff.push_back(ip); savail.push_back(clen); doff.push_back(op); dlen.push_back(olen); csz.push_back(clen); }
-        hoff.push_back(op); hlen.push_back(olen); want.push_back(check);
-        ip += (size_t)clen; op += (size_t)olen;
-    }
+    b200::Lz4BlockHostSink sink{ src, dst, b200::Lz4BlockRoom{ cap } };
+    const b200::Lz4BlockEnd e = b200::walk_lz4block(src, n, stopOnEmptyBlock != 0, sink);   // refill (:191-264)
+    // what is wrong with the container itself, behind the blocks taken: the reader would have decoded and checked THOSE
+    // first, so their verdict comes first.  A block that does not fit lies before anything the walk met later.
+    const int64_t tail = sink.room.full ? -9 : e.err;
     // per block the reader decodes, compares the consumed length, then the checksum -- all "Stream is corrupted" (:236-262)
-    if (!soff.empty()) {
-        std::vector<int32_t> res(soff.size());
-        int rc = b200lz4_decompress_fast_batch_host(src, soff.data(), savail.data(), dst, doff.data(), dlen.data(), res.data(), soff.size());
+    if (!sink.soff.empty()) {
+        std::vector<int32_t> res(sink.soff.size());
+        int rc = b200lz4_decompress_fast_batch_host(src, sink.soff.data(), sink.savail.data(), dst, sink.doff.data(), sink.dlen.data(),
+                                                    res.data(), sink.soff.size());
         if (rc) return rc;
-        for (size_t i = 0; i < res.size(); i++) if (res[i] != csz[i]) return -2;  // compressedLen != compressedLen2 (:247-250)
+        for (size_t i = 0; i < res.size(); i++) if (res[i] != sink.savail[i]) return -2;   // compressedLen != compressedLen2 (:247-250)
     }
-    if (!hoff.empty()) {
-        std::vector<uint32_t> sums(hoff.size());
-        int rc = b200xxh32_batch_host(dst, hoff.data(), hlen.data(), LZ4BLOCK_SEED, sums.data(), hoff.size());
+    if (!sink.hoff.empty()) {
+        std::vector<uint32_t> sums(sink.hoff.size());
+        int rc = b200xxh32_batch_host(dst, sink.hoff.data(), sink.hlen.data(), b200::LZ4BLOCK_SEED, sums.data(), sink.hoff.size());
         if (rc) return rc;
-        for (size_t i = 0; i < sums.size(); i++) if ((sums[i] & 0x0FFFFFFFu) != want[i]) return -2;
+        for (size_t i = 0; i < sums.size(); i++) if ((sums[i] & 0x0FFFFFFFu) != sink.want[i]) return -2;
     }
     if (tail) return tail;
-    if (srcConsumed) *srcConsumed = ip;
-    return (int64_t)op;
+    if (srcConsumed) *srcConsumed = e.ip;
+    return (int64_t)sink.room.used;
+}
+
+int b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int stopOnEmptyBlock,
+                                int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream)
+{
+    return b200::lz4block_decompress_dev(d_src, src_off, src_len, ns, d_dst, dst_off, dst_cap, stopOnEmptyBlock != 0, result,
+                                         src_consumed, content_len, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------- length-prefixed block (LZ4CompressorWithLength.java:45-50)

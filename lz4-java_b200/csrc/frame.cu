@@ -28,9 +28,6 @@
 
 namespace b200 {
 
-cudaError_t launch_gather(const uint8_t* src, const uint64_t* src_off, const int32_t* lens,
-                          uint8_t* dst, const uint64_t* dst_off, size_t n, cudaStream_t st);
-
 struct FrameRec {
     uint64_t desc_off; int32_t desc_len; uint8_t hc_byte; uint8_t flg; uint32_t bs;
     uint64_t content_size; bool has_size;

@@ -56,6 +56,9 @@ cudaError_t launch_compact(const uint8_t* slots, const uint64_t* slot_off, const
 // the scan alone: out_off[i] = *carry_in + exclusive prefix of max(lens, 0); *total = *carry_in + the sum (carry_in may be
 // NULL: 0).  carry_in and total must be different words.
 cudaError_t launch_scan(const int32_t* lens, uint64_t* out_off, uint64_t* total, const uint64_t* carry_in, size_t n, cudaStream_t st);
+// the gather alone: block i's max(lens[i], 0) bytes move from src + src_off[i] to dst + dst_off[i], one warp each
+cudaError_t launch_gather(const uint8_t* src, const uint64_t* src_off, const int32_t* lens,
+                          uint8_t* dst, const uint64_t* dst_off, size_t n, cudaStream_t st);
 
 // ---- LZ4 Frame writer (frame_encode.cu, driven by compress_frames_dev in containers.cu for b200lz4f_compress_dev, and for
 // b200lz4f_compress_host_hc on a device copy of its source).  flags: bit0 content checksum, bit1 block checksums, bit2
@@ -74,6 +77,7 @@ struct FramePlan {
     const uint64_t* f_len; const uint32_t* f_sum;                   // per frame: content size, content checksum (flags bit 0)
     uint64_t* f_off; uint64_t* f_end;                               //   where it starts and ends in dst
     uint32_t nitems; int bsCode; int flags;
+    int level;                                                      // LZ4Block streams: the token's level nibble
 };
 // items [i0, i0 + n): their sizes (frame_size_kernel), and their block words and payloads (frame_emit_kernel, one warp each)
 cudaError_t launch_frame_sizes(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
@@ -173,6 +177,82 @@ cudaError_t launch_frame_walk(const uint8_t* src, uint64_t n, bool single, const
 // walker j's lens[j] records move from recs + segs[j].rec_off to packed + pos[j]
 cudaError_t launch_frame_pack(const WalkSeg* segs, const int32_t* lens, const uint64_t* pos, const WalkRec* recs, WalkRec* packed,
                               uint32_t m, cudaStream_t st);
+
+// ---- "LZ4Block" streams (LZ4BlockOutputStream.java:203-266, LZ4BlockInputStream.java:191-264).  The writer is the frame
+// writer's loop (compress_blocks_dev in containers.cu) with lz4block.cu's item sizes, emit and seal: the same FramePlan, a
+// "frame" being one stream, its last item carrying the empty end block.
+static constexpr int LZ4BLOCK_HEADER = 8 + 1 + 4 + 4 + 4;          // magic, token, compressed and original length, checksum
+static constexpr int LZ4BLOCK_RAW = 0x10, LZ4BLOCK_LZ4 = 0x20;     // the token's method nibble
+static constexpr uint32_t LZ4BLOCK_SEED = 0x9747b28cu;             // LZ4BlockOutputStream.java:56
+static constexpr uint32_t LZ4BLOCK_MAGIC_LO = 0x42345A4Cu, LZ4BLOCK_MAGIC_HI = 0x6B636F6Cu;   // "LZ4Block", little endian
+cudaError_t launch_lz4block_sizes(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
+cudaError_t launch_lz4block_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
+// every item: block checksums (b_sum, masked to 28 bits), end blocks, f_off / f_end
+cudaError_t launch_lz4block_seal(const FramePlan& p, cudaStream_t st);
+
+// The reader's walk of one stream, src[0, n), LZ4BlockInputStream.refill's header rules (:191-264).  Per block whose payload
+// is complete the sink gets block(payload offset, raw, compressed length, original length, checksum).  Returns where the walk
+// stopped and why: err 0 at the end of the stream (the first empty block with `stop`; without it, the end of src, quietly also
+// inside a header, :193-194), -1 premature end, -2 "Stream is corrupted".  Capacity is not the walk's: see Lz4BlockRoom.
+struct Lz4BlockEnd { uint64_t ip; int err; };
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Sink>
+__host__ __device__ inline Lz4BlockEnd walk_lz4block(const uint8_t* src, uint64_t n, bool stop, Sink& sink)
+{
+    uint64_t ip = 0;
+    for (;;) {
+        if (n - ip < (uint64_t)LZ4BLOCK_HEADER) return stop ? Lz4BlockEnd{ ip, -1 } : Lz4BlockEnd{ n, 0 };
+        const uint8_t* h = src + ip;
+        if (rd32(h) != LZ4BLOCK_MAGIC_LO || rd32(h + 4) != LZ4BLOCK_MAGIC_HI) return { ip, -2 };
+        const int token = h[8], method = token & 0xF0, level = 10 + (token & 0x0F);
+        if (method != LZ4BLOCK_RAW && method != LZ4BLOCK_LZ4) return { ip, -2 };
+        const int32_t clen = (int32_t)rd32(h + 9), olen = (int32_t)rd32(h + 13);
+        const uint32_t check = rd32(h + 17);
+        if (olen > (1 << level) || olen < 0 || clen < 0 || (olen == 0 && clen != 0) || (olen != 0 && clen == 0) ||
+            (method == LZ4BLOCK_RAW && olen != clen)) return { ip, -2 };
+        ip += LZ4BLOCK_HEADER;
+        if (olen == 0) {                                                        // empty block (:225-233)
+            if (check != 0) return { ip, -2 };
+            if (stop) return { ip, 0 };
+            continue;
+        }
+        if (n - ip < (uint64_t)clen) return { ip, -1 };
+        sink.block(ip, method == LZ4BLOCK_RAW, clen, olen, check);
+        ip += (uint64_t)clen;
+    }
+}
+// dst_cap applied behind the walk, the same way by both readers: blocks are taken while the prefix sum of their original
+// lengths fits; the first one that does not is the stream's -9 (unless a block before it fails its decode or checksum: -2).
+struct Lz4BlockRoom {
+    uint64_t cap, used = 0; bool full = false;
+    __host__ __device__ bool take(int32_t olen)
+    {
+        if (full || cap - used < (uint64_t)olen) { full = true; return false; }
+        used += (uint64_t)olen;
+        return true;
+    }
+};
+
+// The device reader (lz4block_decompress_dev in containers.cu), all device pointers.  Per stream: its bytes and room, what the
+// counting walk found, where its records go (exclusive prefixes of the counts) and the results.  Per block that fits, in
+// stream order: b_*; per compressed block c_*, per stored block r_* (BatchArgs of the fast decoder and of the gather).
+struct Lz4BlockRead {
+    const uint8_t* src;
+    const uint64_t *s_off, *s_len, *d_off, *d_cap;
+    int32_t *n_comp, *n_raw, *tail; uint64_t *ip, *content;             // the counting walk (tail: -9 when a block does not fit)
+    const uint64_t *p_comp, *p_raw;
+    int64_t* result; uint64_t* consumed;
+    uint64_t *c_soff, *c_doff; int32_t *c_clen, *c_olen, *c_res;
+    uint64_t *r_soff, *r_doff; int32_t* r_len;
+    uint64_t* b_doff; int32_t *b_len, *b_comp; uint32_t *b_want, *b_sum;
+    uint32_t ns; bool stop;
+};
+// one thread per stream: with `record` false the counts, tail, ip and content; with it the records of the blocks that fit
+cudaError_t launch_lz4block_walk(const Lz4BlockRead& r, bool record, cudaStream_t st);
+// one warp per stream: result, consumed
+cudaError_t launch_lz4block_verdict(const Lz4BlockRead& r, cudaStream_t st);
 
 // Average buffer length from which the hash batches give each buffer a whole warp (launch_xxh*_long) instead of a lane.
 static constexpr uint64_t XXH_LONG_AVG = 32768;

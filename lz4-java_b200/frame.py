@@ -164,6 +164,73 @@ def decompress_lz4block(src, max_decoded: int, stop_on_empty_block: bool = True)
     return out[:r].tobytes()
 
 
+def _dev_streams(src, src_off, src_len, what):
+    """the host offset / length arrays of a device call over streams of src, checked against it"""
+    import torch
+    off = np.ascontiguousarray(np.asarray(src_off, dtype=np.uint64).reshape(-1))
+    ln = np.ascontiguousarray(np.asarray(src_len, dtype=np.uint64).reshape(-1))
+    if len(off) != len(ln):
+        raise ValueError("src_off and src_len must have the same length")
+    if not isinstance(src, torch.Tensor) or src.dtype != torch.uint8 or not src.is_cuda or not src.is_contiguous():
+        raise ValueError("src must be a contiguous uint8 CUDA tensor")
+    if len(ln) and int((off + ln).max()) > src.numel():
+        raise ValueError(f"a {what} reaches past the end of src")
+    return off, ln
+
+
+def compress_lz4block_dev(src, src_off, src_len, block_size: int = 1 << 16, hc_level: int = 0, out=None):
+    """independent LZ4Block streams of bytes already in device memory, written on the device (b200lz4block_compress_dev):
+    stream s is src[src_off[s] : src_off[s] + src_len[s]], byte for byte what compress_lz4block writes for the same bytes at
+    the same 16-byte phase.  src: a uint8 CUDA tensor; src_off / src_len: host sequences; out: a uint8 CUDA tensor on src's
+    device (default: a new one of the summed stream bounds).  Runs on torch's current stream and returns when the streams
+    are written.  -> (out[:total], stream_off, stream_len), the last two np.uint64 arrays (where each stream lies in out)"""
+    import torch
+    off, ln = _dev_streams(src, src_off, src_len, "stream")
+    L = N.lib()
+    if L.b200lz4block_compress_bound(0, block_size) == 0:
+        raise ValueError("blockSize must be >= 64 and <= 32 MiB")            # LZ4BlockOutputStream.java:58-66
+    bound = sum(L.b200lz4block_compress_bound(int(n), block_size) for n in ln)
+    if out is None:
+        out = torch.empty(max(bound, 1), dtype=torch.uint8, device=src.device)
+    elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    stream_off, stream_len = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
+    r = L.b200lz4block_compress_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(), out.numel(),
+                                    stream_off.ctypes.data, stream_len.ctypes.data, block_size, hc_level,
+                                    torch.cuda.current_stream(src.device).cuda_stream)
+    N.check(r)
+    if r < 0:
+        raise LZ4FrameError(int(r))
+    return out[:r], stream_off, stream_len
+
+
+def decompress_lz4block_dev(src, src_off, src_len, out, dst_off, dst_cap, stop_on_empty_block: bool = True):
+    """many LZ4Block streams in device memory, each read as its own LZ4BlockInputStream(in, stopOnEmptyBlock) into device
+    memory (b200lz4block_decompress_dev): stream s is src[src_off[s] : src_off[s] + src_len[s]], decoded to out[dst_off[s]:]
+    with room for dst_cap[s] bytes.  No byte of the streams or the content crosses to the host.  src, out: contiguous uint8
+    CUDA tensors on one device; the offsets and lengths: host sequences.  Runs on torch's current stream and returns when the
+    results are on the host.  -> (result, src_consumed, content_len), np.int64 / np.uint64 / np.uint64 arrays: per stream
+    what decompress_lz4block would return (decoded bytes, or -1 premature end, -2 corrupted, -9 room too small), how far it
+    read (0 on an error), and what it decodes to when room is not the limit.  Raises only on a backend error."""
+    import torch
+    off, ln = _dev_streams(src, src_off, src_len, "stream")
+    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+    if len(doff) != len(ln) or len(dcap) != len(ln):
+        raise ValueError("dst_off and dst_cap must have one entry per stream")
+    if len(ln) and int((doff + dcap).max()) > out.numel():
+        raise ValueError("a destination range reaches past the end of out")
+    result = np.zeros(len(ln), dtype=np.int64)
+    consumed, content = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
+    N.check(N.lib().b200lz4block_decompress_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
+                                                doff.ctypes.data, dcap.ctypes.data, int(bool(stop_on_empty_block)),
+                                                result.ctypes.data, consumed.ctypes.data, content.ctypes.data,
+                                                torch.cuda.current_stream(src.device).cuda_stream))
+    return result, consumed, content
+
+
 # ---- LZ4CompressorWithLength / LZ4DecompressorWithLength
 def compress_with_length(src) -> bytes:
     s = _view(src)
