@@ -319,6 +319,39 @@ int     b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_of
 int     b200lz4_compress_with_length(const char* src, char* dst, int srcSize, int dstCapacity);
 int     b200lz4_decompressed_length(const char* src);
 int     b200lz4_decompress_with_length(const char* src, int srcAvail, char* dst, int dstCapacity);
+/* LZ4DecompressorWithLength(LZ4SafeDecompressor) (lz4-java 1.8, LZ4DecompressorWithLength.java:148-154): src is exactly one
+ * record of srcLen bytes.  -1 when srcLen < 4, or the declared length is negative or larger than dstCapacity; otherwise
+ * b200lz4_decompress_safe(src + 4, dst, srcLen - 4, declared): the bytes decoded, or < 0. */
+int     b200lz4_decompress_with_length_safe(const char* src, int srcLen, char* dst, int dstCapacity);
+
+/* Device-resident LZ4CompressorWithLength (LZ4CompressorWithLength.java:45-50) for n independent records.  Record r is
+ * src_len[r] bytes at d_src + src_off[r] (HOST arrays; the bytes are in device memory of the current device); the records are
+ * written back to back into d_dst, rec_off / rec_len (host, may be NULL) say where.  A record is 4 bytes of little-endian
+ * src_len[r], then one LZ4 block of the whole record.  hc_level 0 = the fast compressor: each record is byte for byte what
+ * b200lz4_compress_with_length writes for the same bytes at the same 16-byte phase (the compressor is picked per record by its
+ * length, as that call picks it).  1..17 = LZ4_compress_HC at that level: the block is what b200lz4_compress_HC writes.
+ * Returns the total bytes written, or: -9 dst_capacity < sum of b200lz4_compressBound(src_len[r]) + 4; B200LZ4_E_ARG
+ * (a record longer than 0x7E000000 bytes, a NULL pointer where bytes are needed), _CUDA, _NODEVICE.  Argument and size errors
+ * are found before anything is launched or written.  Ordered after the work already queued on `stream`; returns when the
+ * records are in d_dst.  Grow-or-keep scratch of the thread's context: the frame writer's. */
+int64_t b200lz4_compress_with_length_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
+                                         uint8_t* d_dst, size_t dst_capacity, uint64_t* rec_off, uint64_t* rec_len,
+                                         int hc_level, void* stream);
+
+/* Device-resident LZ4DecompressorWithLength for n independent records, HBM to HBM.  Record r is the src_len[r] readable bytes
+ * at d_src + src_off[r] (at most 2^31 - 1), decoded to d_dst + dst_off[r] with room dst_cap[r] (all offset / length arrays HOST,
+ * the bytes device memory of the current device).  safe == 0, the LZ4FastDecompressor flavour: result[r] is what
+ * b200lz4_decompress_with_length(src, src_len, dst, dst_cap) returns (the bytes read including the prefix, or < 0);
+ * safe != 0, the LZ4SafeDecompressor flavour: what b200lz4_decompress_with_length_safe returns (the bytes decoded, or < 0).
+ * orig_len[r] (may be NULL): the declared length, -1 when src_len[r] < 4; a record refused for want of room can be read again
+ * with dst_cap[r] = orig_len[r].  Nothing outside [dst_off[r], dst_off[r] + dst_cap[r]) is written, nothing at all for a
+ * record its header rejects, and on success nothing past dst_off[r] + the declared length (fast) or + result[r] (safe).
+ * Three launches whatever n is; only the per-record arguments go up and the results come back.  Returns 0 or B200LZ4_E_*.
+ * Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep scratch of the
+ * thread's context: the frame reader's. */
+int     b200lz4_decompress_with_length_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
+                                           uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int safe,
+                                           int64_t* result, int64_t* orig_len, void* stream);
 
 /* kernel-launch counter (bench.py's "gpu_launches"): number of kernels this library has
  * launched from the calling process since load / since the last reset. */

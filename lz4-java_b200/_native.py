@@ -88,6 +88,9 @@ SYMBOLS = [
     ("b200lz4_compress_with_length", _i, [_vp, _vp, _i, _i]),
     ("b200lz4_decompressed_length", _i, [_vp]),
     ("b200lz4_decompress_with_length", _i, [_vp, _i, _vp, _i]),
+    ("b200lz4_decompress_with_length_safe", _i, [_vp, _i, _vp, _i]),
+    ("b200lz4_compress_with_length_dev", C.c_int64, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _i, _vp]),
+    ("b200lz4_decompress_with_length_dev", _i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     ("b200lz4_launch_count", _u64, []),
     ("b200lz4_launch_count_reset", None, []),
     ("b200lz4_context_count", _i, []),

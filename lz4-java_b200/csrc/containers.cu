@@ -4,16 +4,18 @@
 //   * "LZ4Block" container — LZ4BlockOutputStream.flushBufferedData/finish (:203-266) and
 //                            LZ4BlockInputStream.refill (LZ4BlockInputStream.java:191-264)
 //   * length-prefixed block — LZ4CompressorWithLength / LZ4DecompressorWithLength
-// The reference does these one block per native call.  Here both containers are written on the device, by one loop
-// (compress_blocks_dev) with the kernels of frame_encode.cu and lz4block.cu; the host writers run it on a device copy of their
-// source.  The LZ4Block reader walks the headers with walk_lz4block (kernels.h): on the host for host buffers, whose payload
-// work (block decompression, every XXH32) goes through the batch entry points, and on the device for streams in device
-// memory (lz4block.cu).  No hashing or codec arithmetic runs on the host.
+// The reference does these one block per native call.  Here all three containers are written on the device, by one loop
+// (compress_blocks_dev) with the kernels of frame_encode.cu, lz4block.cu and with_length.cu; the host writers run it on a
+// device copy of their source.  The LZ4Block reader walks the headers with walk_lz4block (kernels.h): on the host for host
+// buffers, whose payload work (block decompression, every XXH32) goes through the batch entry points, and on the device for
+// streams in device memory (lz4block.cu).  Length-prefixed records in device memory are read by with_length.cu's kernels
+// around the block decoders.  No hashing or codec arithmetic runs on the host.
 #include "../../include/b200lz4.h"
 #include "kernels.h"
-#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device writers' and reader's kernels come with it
+#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device writers' and readers' kernels come with it
 #include "frame_encode.cu"
 #include "lz4block.cu"
+#include "with_length.cu"
 #endif
 #include <cstdlib>
 #include <cstring>
@@ -42,20 +44,24 @@ struct FramePlanLayout {
     }
 };
 
-struct FrameChunk { size_t i0, i1, b0, b1; };                       // items [i0, i1), their blocks [b0, b1)
+// items [i0, i1), their blocks [b0, b1): the fast compressor's wide kernel takes [b0, bw), its long kernel [bw, b1)
+struct FrameChunk { size_t i0, i1, b0, b1, bw; };
 
-// The two containers written on the device.  An LZ4Block "frame" is one stream: blocks of blockSize bytes, the end block on
-// its last item, checksums of the original blocks.
-enum class Container { Frame, LZ4Block };
+// The three containers written on the device.  An LZ4Block "frame" is one stream: blocks of blockSize bytes, the end block on
+// its last item, checksums of the original blocks.  A WithLength "frame" is one record: one item and one block of its whole
+// length, an empty record included.
+enum class Container { Frame, LZ4Block, WithLength };
 
-// Both writers: arguments and sizes (nothing is launched or written before these pass), the plan, the chunk loop and the
-// results.  Only the item sizes, the emit, the checksums and the seal differ by container.  bs: bytes per block; code:
-// the frame's bsCode or the LZ4Block token's level nibble; flags: the frame's (0 for LZ4Block).
+static constexpr uint64_t LZ4_MAX_INPUT = 0x7E000000;              // LZ4_MAX_INPUT_SIZE (lz4.h:211)
+
+// Every writer: arguments and sizes (nothing is launched or written before these pass), the plan, the chunk loop and the
+// results.  Only the item sizes, the emit, the checksums and the seal differ by container.  bs: bytes per block (WithLength:
+// more than any record); code: the frame's bsCode or the LZ4Block token's level nibble; flags: the frame's (0 otherwise).
 static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
                                    size_t nf, uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
                                    uint64_t bs, int code, int flags, int hc_level, cudaStream_t st)
 {
-    const bool frame = kind == Container::Frame;
+    const bool frame = kind == Container::Frame, rec = kind == Container::WithLength;
     if (nf == 0) return 0;
     if (!src_off || !src_len || !d_dst) return fail_arg("null pointer");
     uint64_t need = 0, nb = 0, ni = 0, bytes = 0;
@@ -63,8 +69,10 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
     for (size_t f = 0; f < nf; f++) {
         const uint64_t n = src_len[f];
         if (n > (1ull << 47)) return fail_arg("src_len");
-        need += frame ? b200lz4f_compress_bound(n, code) : b200lz4block_compress_bound(n, (int)bs);
-        nb += (n + bs - 1) / bs; ni += n ? (n + bs - 1) / bs : 1; bytes += n;
+        if (rec && n > LZ4_MAX_INPUT) return fail_arg("a record is at most 0x7E000000 bytes");
+        const uint64_t nbf = rec ? 1 : (n + bs - 1) / bs;
+        need += frame ? b200lz4f_compress_bound(n, code) : rec ? 4 + compress_bound(n) : b200lz4block_compress_bound(n, (int)bs);
+        nb += nbf; ni += nbf ? nbf : 1; bytes += n;
         if ((flags & 1) && n > 0x7FFFFFFFull) too_long = true;
     }
     if (bytes && !d_src) return fail_arg("null pointer");
@@ -85,13 +93,37 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
     std::vector<FrameChunk> chunks;
     size_t b = 0, i = 0, ci0 = 0, cb0 = 0;
     uint64_t slot = 0, span = 0, slots_need = 0;
+    // A chunk's blocks go to the wide compressor when they are at most 64 KiB (as b200lz4_compress_default picks it), else to
+    // the long one.  Frame and LZ4Block blocks are all of one class.  Records are of either: the records of up to 64 KiB are
+    // moved to the front of the chunk's blocks, so each class is one contiguous range and one launch; the items, and so the
+    // scan and the output, stay in record order.
+    auto close_chunk = [&](size_t i1) {
+        size_t bw = bs <= 65536 ? b : cb0;
+        if (rec) {
+            struct Row { uint64_t soff, slot; int32_t slen, ccap; };
+            std::vector<Row> rows(b - cb0);                             // block cb0 + k is item ci0 + k's
+            for (size_t k = 0; k < rows.size(); k++)
+                rows[k] = Row{ h64(L.b_soff)[cb0 + k], h64(L.b_slot)[cb0 + k], h32(L.b_slen)[cb0 + k], h32(L.b_ccap)[cb0 + k] };
+            size_t w = cb0;
+            for (int wide = 1; wide >= 0; wide--) {
+                for (size_t k = 0; k < rows.size(); k++) {
+                    if ((rows[k].slen <= 65536) != (wide == 1)) continue;
+                    h64(L.b_soff)[w] = rows[k].soff; h64(L.b_slot)[w] = rows[k].slot;
+                    h32(L.b_slen)[w] = rows[k].slen; h32(L.b_ccap)[w] = rows[k].ccap;
+                    h32(L.i_block)[ci0 + k] = (int32_t)w; w++;
+                }
+                if (wide) bw = w;
+            }
+        }
+        chunks.push_back(FrameChunk{ ci0, i1, cb0, b, bw });
+    };
     for (size_t f = 0; f < nf; f++) {
-        const uint64_t n = src_len[f], nbf = (n + bs - 1) / bs;
+        const uint64_t n = src_len[f], nbf = rec ? 1 : (n + bs - 1) / bs;
         h64(L.f_soff)[f] = src_off[f]; h64(L.f_len)[f] = n; h32(L.f_len32)[f] = (int32_t)(n < 0x7FFFFFFFull ? n : 0x7FFFFFFFull);
         for (uint64_t k = 0; k < (nbf ? nbf : 1); k++, i++) {
             const uint64_t len = nbf ? (n - k * bs < bs ? n - k * bs : bs) : 0;
             if (i > ci0 && (i - ci0 >= CHUNK_BLOCKS || span + len > CHUNK_SPAN)) {
-                chunks.push_back(FrameChunk{ ci0, i, cb0, b });
+                close_chunk(i);
                 slots_need = slot > slots_need ? slot : slots_need;
                 ci0 = i; cb0 = b; slot = 0; span = 0;
             }
@@ -103,7 +135,7 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
             slot += aligned_compress_bound(len); span += len; b++;
         }
     }
-    chunks.push_back(FrameChunk{ ci0, i, cb0, b });
+    close_chunk(i);
     slots_need = slot > slots_need ? slot : slots_need;
     h64(L.carry)[0] = 0;
     rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
@@ -122,8 +154,8 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
     auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
     // checksums of the sources alone, so from the start, beside everything else: the frame's content checksums, or the
-    // LZ4Block checksums of the original blocks
-    const bool early_sums = frame ? (flags & 1) != 0 : nb > 0;
+    // LZ4Block checksums of the original blocks (records have none)
+    const bool early_sums = frame ? (flags & 1) != 0 : !rec && nb > 0;
     if (early_sums) {
         CK(cudaEventRecord(side->fork, st));
         CK(cudaStreamWaitEvent(side->st, side->fork, 0));
@@ -135,24 +167,29 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
                 d_src, P.b_soff, P.b_slen, LZ4BLOCK_SEED, (uint32_t*)P.b_sum, (size_t)nb, side->st)));
         CK(cudaEventRecord(side->join, side->st));
     }
+    auto blocks = [&](size_t b0, size_t b1) {
+        return BatchArgs{ d_src, P.b_soff + b0, P.b_slen + b0, s->d_slots, P.b_slot + b0,
+                          (const int32_t*)(D + L.b_ccap) + b0, (int32_t*)P.b_clen + b0, b1 - b0 };
+    };
     for (size_t k = 0; k < chunks.size(); k++) {
         const FrameChunk& c = chunks[k];
-        if (c.b1 > c.b0) {          // the stream's compressor argument: hc_level 0 = the fast compressor, 1..17 = HC
-            const BatchArgs a{ d_src, P.b_soff + c.b0, P.b_slen + c.b0, s->d_slots, P.b_slot + c.b0,
-                               (const int32_t*)(D + L.b_ccap) + c.b0, (int32_t*)P.b_clen + c.b0, c.b1 - c.b0 };
-            CK(counted(hc_level > 0 ? launch_compress_hc(a, hc_level, st) : launch_compress_fast(a, bs <= 65536 ? 65536 : 0, st)));
-        }
+        // the stream's compressor argument: hc_level 0 = the fast compressor, 1..17 = HC
+        if (hc_level > 0 && c.b1 > c.b0) CK(counted(launch_compress_hc(blocks(c.b0, c.b1), hc_level, st)));
+        if (hc_level <= 0 && c.bw > c.b0) CK(counted(launch_compress_fast(blocks(c.b0, c.bw), 65536, st)));
+        if (hc_level <= 0 && c.b1 > c.bw) CK(counted(launch_compress_fast(blocks(c.bw, c.b1), 0, st)));
         const uint32_t i0 = (uint32_t)c.i0, n = (uint32_t)(c.i1 - c.i0);
-        CK(counted(frame ? launch_frame_sizes(P, i0, n, st) : launch_lz4block_sizes(P, i0, n, st)));
+        CK(counted(frame ? launch_frame_sizes(P, i0, n, st) : rec ? launch_with_length_sizes(P, i0, n, st)
+                                                                  : launch_lz4block_sizes(P, i0, n, st)));
         CK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
-        CK(counted(frame ? launch_frame_emit(P, i0, n, st) : launch_lz4block_emit(P, i0, n, st)));
+        CK(counted(frame ? launch_frame_emit(P, i0, n, st) : rec ? launch_with_length_emit(P, i0, n, st)
+                                                                 : launch_lz4block_emit(P, i0, n, st)));
     }
     if ((flags & 2) && nb) {        // block checksums over the payloads as written; the source average bounds the payloads'
         CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
             d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
     }
     if (early_sums) CK(cudaStreamWaitEvent(st, side->join, 0));
-    CK(counted(frame ? launch_frame_seal(P, st) : launch_lz4block_seal(P, st)));
+    if (!rec) CK(counted(frame ? launch_frame_seal(P, st) : launch_lz4block_seal(P, st)));   // records: the emit placed them
     CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     drain.done = true;
@@ -185,6 +222,14 @@ static int64_t compress_lz4block_dev(const uint8_t* d_src, const uint64_t* src_o
     if (blockSize < 64 || blockSize > (1 << 25)) return fail_arg("blockSize must be 64..32 MiB");
     return compress_blocks_dev(Container::LZ4Block, d_src, src_off, src_len, ns, d_dst, dst_capacity, stream_off, stream_len,
                                (uint64_t)blockSize, lz4block_level(blockSize), 0, hc_level, st);
+}
+
+static int64_t compress_with_length_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
+                                        uint8_t* d_dst, size_t dst_capacity, uint64_t* rec_off, uint64_t* rec_len, int hc_level,
+                                        cudaStream_t st)
+{   // one block per record: bs is longer than any record may be
+    return compress_blocks_dev(Container::WithLength, d_src, src_off, src_len, n, d_dst, dst_capacity, rec_off, rec_len,
+                               1ull << 31, 0, 0, hc_level, st);
 }
 
 // A device writer, write(d_src, src_off, src_len, d_dst, capacity, st) for one source, run on a copy of src in the thread's
@@ -312,6 +357,69 @@ static int lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off
     memcpy(result, H + L.result, 8 * ns);
     if (src_consumed) memcpy(src_consumed, H + L.consumed, 8 * ns);
     if (content_len) memcpy(content_len, H + L.content, 8 * ns);
+    return 0;
+}
+
+// ---------------------------------------------------------------- length-prefixed records in device memory (with_length.cu)
+// Where one call's per-record arrays lie in the reader scratch's d_seg / h_seg: the arguments go up, the results come back,
+// the decoder's arguments and results stay on the device.
+struct WithLengthLayout {
+    size_t s_off, s_len, d_off, d_cap, b_soff, b_slen, b_dlen, b_res, head, result, orig, bytes = 0;
+    explicit WithLengthLayout(size_t n)
+    {
+        auto take = [&](size_t k) { const size_t at = bytes; bytes = (bytes + k + 15) & ~size_t(15); return at; };
+        s_off = take(8 * n); s_len = take(8 * n); d_off = take(8 * n); d_cap = take(8 * n);
+        b_soff = take(8 * n); b_slen = take(4 * n); b_dlen = take(4 * n); b_res = take(4 * n); head = take(4 * n);
+        result = take(8 * n); orig = take(8 * n);
+    }
+};
+
+// The header kernel, the fast or safe decoder over every record, the verdict kernel: three launches whatever n is, and one
+// synchronisation.
+static int with_length_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
+                                      uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, bool safe,
+                                      int64_t* result, int64_t* orig_len, cudaStream_t st)
+{
+    if (n == 0) return 0;
+    if (!src_off || !src_len || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
+    if (n > 0x7FFFFFFFull) return fail_arg("too many records in one call");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < n; k++) {
+        if (src_len[k] > 0x7FFFFFFFull) return fail_arg("src_len: a record is at most 2^31 - 1 bytes");
+        if (dst_cap[k] > (1ull << 47)) return fail_arg("dst_cap");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    FrameReadScratch* s;
+    int rc = get_frame_read_scratch(&s);
+    const WithLengthLayout L(n);
+    if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
+    if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
+    if (rc) return rc;
+    uint8_t *D = s->d_seg, *H = s->h_seg;
+    memcpy(H + L.s_off, src_off, 8 * n); memcpy(H + L.s_len, src_len, 8 * n);
+    memcpy(H + L.d_off, dst_off, 8 * n); memcpy(H + L.d_cap, dst_cap, 8 * n);
+    WithLengthRead r{};
+    r.src = d_src;
+    r.s_off = (const uint64_t*)(D + L.s_off); r.s_len = (const uint64_t*)(D + L.s_len); r.d_cap = (const uint64_t*)(D + L.d_cap);
+    r.b_soff = (uint64_t*)(D + L.b_soff); r.b_slen = (int32_t*)(D + L.b_slen); r.b_dlen = (int32_t*)(D + L.b_dlen);
+    r.b_res = (int32_t*)(D + L.b_res); r.head = (int32_t*)(D + L.head);
+    r.result = (int64_t*)(D + L.result); r.orig_len = (int64_t*)(D + L.orig);
+    r.n = (uint32_t)n; r.safe = safe;
+    // fast: src_len = the readable bytes, dst_cap = the exact decoded size; safe: the block's size and maxDestLen
+    const BatchArgs a{ d_src, r.b_soff, r.b_slen, d_dst, (const uint64_t*)(D + L.d_off), r.b_dlen, r.b_res, n };
+
+    Drain drain{ st };
+    CK(cudaMemcpyAsync(D, H, L.b_soff, cudaMemcpyHostToDevice, st));
+    g_launch_count.fetch_add(3, std::memory_order_relaxed);
+    CK(launch_with_length_head(r, st));
+    CK(safe ? launch_decompress_safe(a, st) : launch_decompress_fast(a, st));
+    CK(launch_with_length_verdict(r, st));
+    CK(cudaMemcpyAsync(H + L.result, D + L.result, L.bytes - L.result, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    memcpy(result, H + L.result, 8 * n);
+    if (orig_len) memcpy(orig_len, H + L.orig, 8 * n);
     return 0;
 }
 
@@ -450,6 +558,31 @@ int b200lz4_decompress_with_length(const char* src, int srcAvail, char* dst, int
     if (n < 0 || n > dstCapacity) return -1;
     const int r = b200lz4_decompress_fast_bounded(src + 4, srcAvail - 4, dst, n);
     return r < 0 ? r : r + 4;
+}
+// safe-decompressor flavour (lz4-java 1.8): src is exactly one record; returns the bytes decoded or < 0
+// (LZ4DecompressorWithLength.java:148-154)
+int b200lz4_decompress_with_length_safe(const char* src, int srcLen, char* dst, int dstCapacity)
+{
+    if (srcLen < 4) return -1;
+    const int n = b200lz4_decompressed_length(src);
+    if (n < 0 || n > dstCapacity) return -1;
+    return b200lz4_decompress_safe(src + 4, dst, srcLen - 4, n);
+}
+
+int64_t b200lz4_compress_with_length_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
+                                         uint8_t* d_dst, size_t dst_capacity, uint64_t* rec_off, uint64_t* rec_len,
+                                         int hc_level, void* stream)
+{
+    return b200::compress_with_length_dev(d_src, src_off, src_len, n, d_dst, dst_capacity, rec_off, rec_len, hc_level,
+                                          (cudaStream_t)stream);
+}
+
+int b200lz4_decompress_with_length_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
+                                       uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int safe,
+                                       int64_t* result, int64_t* orig_len, void* stream)
+{
+    return b200::with_length_decompress_dev(d_src, src_off, src_len, n, d_dst, dst_off, dst_cap, safe != 0, result, orig_len,
+                                            (cudaStream_t)stream);
 }
 
 } // extern "C"

@@ -254,6 +254,27 @@ cudaError_t launch_lz4block_walk(const Lz4BlockRead& r, bool record, cudaStream_
 // one warp per stream: result, consumed
 cudaError_t launch_lz4block_verdict(const Lz4BlockRead& r, cudaStream_t st);
 
+// ---- length-prefixed records (LZ4CompressorWithLength / LZ4DecompressorWithLength).  The writer is the frame writer's loop
+// (compress_blocks_dev) with with_length.cu's item sizes and emit: a "frame" is one record, one item and one block of its
+// whole length (an empty record too).  The emit also writes f_off / f_end, so there is no seal.
+cudaError_t launch_with_length_sizes(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
+cudaError_t launch_with_length_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
+
+// The device reader (with_length_decompress_dev in containers.cu), all device pointers.  Per record: its bytes and room, the
+// decoder's arguments (BatchArgs of the fast or safe decoder, dst_off being d_off), the header's verdict and the results.
+struct WithLengthRead {
+    const uint8_t* src;
+    const uint64_t *s_off, *s_len, *d_cap;
+    uint64_t* b_soff; int32_t *b_slen, *b_dlen, *b_res;
+    int32_t* head;                                                      // 0, or -1 when the header rejects the record
+    int64_t *result, *orig_len;
+    uint32_t n; bool safe;
+};
+// one thread per record: head, orig_len and the decoder's arguments
+cudaError_t launch_with_length_head(const WithLengthRead& r, cudaStream_t st);
+// one thread per record: result
+cudaError_t launch_with_length_verdict(const WithLengthRead& r, cudaStream_t st);
+
 // Average buffer length from which the hash batches give each buffer a whole warp (launch_xxh*_long) instead of a lane.
 static constexpr uint64_t XXH_LONG_AVG = 32768;
 

@@ -244,7 +244,10 @@ def compress_with_length(src) -> bytes:
     return out[:r].tobytes()
 
 
-def decompress_with_length(src) -> bytes:
+def decompress_with_length(src, safe: bool = False) -> bytes:
+    """LZ4DecompressorWithLength.decompress(src).  safe=False: the LZ4FastDecompressor flavour, src[4:] is read as far as the
+    declared length needs; safe=True: the LZ4SafeDecompressor flavour of lz4-java 1.8 (LZ4DecompressorWithLength.java:148-154),
+    src is exactly one record and the decoded bytes are returned, at most the declared length of them."""
     s = _view(src)
     from .lz4 import LZ4Exception
     if len(s) < 4:
@@ -253,8 +256,66 @@ def decompress_with_length(src) -> bytes:
     if n < 0:
         raise LZ4Exception("negative length")
     out = np.empty(max(n, 1), dtype=np.uint8)
+    if safe:
+        r = N.lib().b200lz4_decompress_with_length_safe(s.ctypes.data, len(s), out.ctypes.data, n)
+        N.check(r)
+        if r < 0:
+            raise LZ4Exception("Error decoding offset " + str(4 - r) + " of input buffer")   # LZ4JNISafeDecompressor.java:39-41
+        return out[:r].tobytes()
     r = N.lib().b200lz4_decompress_with_length(s.ctypes.data, len(s), out.ctypes.data, n)
     N.check(r)
     if r < 0:
         raise LZ4Exception("Error decoding offset " + str(-r) + " of input buffer")
     return out[:n].tobytes()
+
+
+def compress_with_length_dev(src, src_off, src_len, hc_level: int = 0, out=None):
+    """independent length-prefixed records (LZ4CompressorWithLength) of bytes already in device memory, written on the device
+    (b200lz4_compress_with_length_dev): record r is src[src_off[r] : src_off[r] + src_len[r]]; with hc_level 0 it is byte for
+    byte what compress_with_length writes for the same bytes at the same 16-byte phase, with 1..17 the length and an
+    LZ4_compress_HC block of that level.  src: a uint8 CUDA tensor; src_off / src_len: host sequences; out: a uint8 CUDA tensor
+    on src's device (default: a new one of the summed record bounds).  Runs on torch's current stream and returns when the
+    records are written.  -> (out[:total], rec_off, rec_len), the last two np.uint64 arrays (where each record lies in out)"""
+    import torch
+    off, ln = _dev_streams(src, src_off, src_len, "record")
+    if len(ln) and int(ln.max()) > 0x7E000000:
+        raise ValueError("a record is at most 0x7E000000 bytes (LZ4_MAX_INPUT_SIZE)")
+    bound = int((ln + ln // 255 + 16 + 4).sum())
+    if out is None:
+        out = torch.empty(max(bound, 1), dtype=torch.uint8, device=src.device)
+    elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    rec_off, rec_len = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
+    r = N.lib().b200lz4_compress_with_length_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
+                                                 out.numel(), rec_off.ctypes.data, rec_len.ctypes.data, hc_level,
+                                                 torch.cuda.current_stream(src.device).cuda_stream)
+    N.check(r)
+    if r < 0:
+        raise LZ4FrameError(int(r))
+    return out[:r], rec_off, rec_len
+
+
+def decompress_with_length_dev(src, src_off, src_len, out, dst_off, dst_cap, safe: bool = False):
+    """many length-prefixed records in device memory, each read by LZ4DecompressorWithLength into device memory
+    (b200lz4_decompress_with_length_dev): record r is src[src_off[r] : src_off[r] + src_len[r]], decoded to out[dst_off[r]:]
+    with room for dst_cap[r] bytes.  safe: the LZ4SafeDecompressor flavour (the record is exactly src_len[r] bytes) rather
+    than the LZ4FastDecompressor one.  No byte of the records or the content crosses to the host.  src, out: contiguous uint8
+    CUDA tensors on one device; the offsets and lengths: host sequences.  Runs on torch's current stream and returns when the
+    results are on the host.  -> (result, orig_len), np.int64 arrays: per record what decompress_with_length's host call
+    returns (fast: the bytes read including the prefix; safe: the bytes decoded; < 0 on an error), and the declared length
+    (-1 when the record is shorter than 4 bytes).  Raises only on a backend error."""
+    import torch
+    off, ln = _dev_streams(src, src_off, src_len, "record")
+    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+    if len(doff) != len(ln) or len(dcap) != len(ln):
+        raise ValueError("dst_off and dst_cap must have one entry per record")
+    if len(ln) and int((doff + dcap).max()) > out.numel():
+        raise ValueError("a destination range reaches past the end of out")
+    result, orig_len = np.zeros(len(ln), dtype=np.int64), np.zeros(len(ln), dtype=np.int64)
+    N.check(N.lib().b200lz4_decompress_with_length_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
+                                                       doff.ctypes.data, dcap.ctypes.data, int(bool(safe)), result.ctypes.data,
+                                                       orig_len.ctypes.data, torch.cuda.current_stream(src.device).cuda_stream))
+    return result, orig_len
