@@ -251,6 +251,29 @@ void*   b200lz4f_index_create_dev(const uint8_t* d_src, size_t srcSize, int sing
  * Ordered after the work already queued on `stream`; returns when d_dst holds the content. */
 int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t srcSize, uint8_t* d_dst, size_t dstCapacity, int single,
                                 const uint64_t* frame_hint, size_t nhint, size_t* src_consumed, void* stream);
+/* Device-resident LZ4 Frame reader for ns independent streams, each read as its own LZ4FrameInputStream(in, readSingleFrame).
+ * Stream s is src_len[s] bytes at d_src + src_off[s], decoded to d_dst + dst_off[s] with room dst_cap[s] (all offset / length
+ * / result arrays HOST; the bytes device memory of the current device).  Source ranges may overlap or leave gaps and start at
+ * any byte.  result[s] is what b200lz4f_decompress_host (single == 0) or b200lz4f_decompress_host_single (single != 0) returns
+ * for the same bytes and dstCapacity = dst_cap[s]: the total, or -1 .. -10 in the same stream order (descriptor hash, then
+ * each block's checksum and decode, then content checksum and content size, frame by frame; then the container's own error
+ * behind them; then -9).  -11 does not occur: the blocks are packed.  src_consumed[s] (may be NULL): where the reader stopped,
+ * what _single reports in *src_consumed; 0 when result[s] < 0.  content_len[s] (may be NULL): what the stream decodes to when
+ * room is not the limit, result[s] on success; after a -9, a call with dst_cap[s] = content_len[s] does not return -9; 0 after
+ * any other error.  A stream with result[s] < 0 writes nothing in d_dst; one that succeeds writes nothing outside
+ * [dst_off[s], dst_off[s] + result[s]): every verdict is in before anything is packed.
+ * Returns 0 or B200LZ4_E_*: NULL pointers where bytes or results are needed, ns above 2^31 - 1 or a destination range that
+ * overflows are found before anything is launched; more than 2^31 - 1 blocks or frames in all (or one stream needing more
+ * than 32 GiB of decode slots) after the first walk, before any payload is touched.  The number of launches does not depend
+ * on ns or on the number of frames or blocks; per stream only its arguments go up and its results come back, and a few
+ * totals in between: no block record crosses to the host.  Each stream is walked by one device thread, twice, so one long
+ * stream of many small blocks is a serial chain of loads; for one large container b200lz4f_decompress_dev with hints is the
+ * better call.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep
+ * scratch of the thread's context: the frame reader's segment buffers, record regions and decode slots (about the content
+ * size rounded up to whole blocks). */
+int     b200lz4f_decompress_streams_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                        uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int single,
+                                        int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream);
 /* Device-resident LZ4 Frame writer (LZ4FrameOutputStream.java:178-251) for nf independent frames, with bsCode / flags /
  * hc_level as b200lz4f_compress_host_hc takes them.  Frame f is src_len[f] bytes at d_src + src_off[f] (src_off / src_len:
  * HOST arrays of nf entries; the bytes are in device memory of the current device).  The frames are written back to back

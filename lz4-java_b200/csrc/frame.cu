@@ -17,8 +17,9 @@
 // device (frame_index.cu) and only its records come to the host; both indexers run the same walk (walk_frames, kernels.h).
 #include "../../include/b200lz4.h"
 #include "kernels.h"
-#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device indexer's kernels come with it
+#ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device readers' kernels come with it
 #include "frame_index.cu"
+#include "frame_streams.cu"
 #endif
 #include <algorithm>
 #include <cstring>
@@ -90,12 +91,10 @@ struct IndexSink {
         BlockRec b{}; b.src_off = src_off; b.size = word & 0x7FFFFFFFu; b.raw = word >> 31; b.frame = ix.frames.size();
         b.has_checksum = f.flg & 0x10;
         if (b.has_checksum) b.checksum = checksum;
-        // the slot: a stored block needs its own size, a compressed one cannot decode to more than 255 bytes per byte
-        // (one length byte adds at most 255) -- so a stream of tiny flushed blocks asks for what it can fill, not for
-        // blockMaxSize each.  Full blocks keep exactly bs: a frame without short blocks in the middle stays contiguous.
-        const uint64_t room = b.raw ? b.size : std::min<uint64_t>(f.bs, 255ull * b.size);
+        // the slot (frame_slot_room, kernels.h)
+        const uint64_t room = frame_slot_room(f.bs, b.size, b.raw);
         b.cap = (uint32_t)room;
-        b.out_off = ix.slot_bytes; ix.slot_bytes += room >= f.bs ? f.bs : ((room + 15) & ~15ull);
+        b.out_off = ix.slot_bytes; ix.slot_bytes += frame_slot_bytes(room, f.bs);
         ix.blocks.push_back(b);
     }
     void frame_end(const WalkFrame& w)
@@ -300,6 +299,141 @@ static int build_descriptors(FrameIndex& ix)
         if (fr.first_block > 0xFFFFFFFFull || fr.nblocks > 0xFFFFFFFFull) return -10;
         ((uint32_t*)(p + L.f_first))[k] = (uint32_t)fr.first_block; ((uint32_t*)(p + L.f_nblk))[k++] = (uint32_t)fr.nblocks;
     }
+    return 0;
+}
+
+// ---- many independent frame streams in device memory (b200lz4f_decompress_streams_dev; kernels: frame_streams.cu)
+// Where one call's per-stream arrays lie in d_seg / h_seg: the arguments and the zeroed `over` word go up; `over` and the
+// scan totals come back after the counting walk, the results at the end.  The counts and their prefixes stay on the device.
+struct FrameStreamLayout {
+    size_t s_off, s_len, d_off, d_cap, over, totals, cnt, pos, tail, ip, result, consumed, content, bytes = 0;
+    explicit FrameStreamLayout(size_t ns)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        s_off = take(8 * ns); s_len = take(8 * ns); d_off = take(8 * ns); d_cap = take(8 * ns);
+        over = take(4); totals = take(8 * FS_ROWS);
+        cnt = take(4 * FS_ROWS * ns); pos = take(8 * FS_ROWS * ns); tail = take(4 * ns); ip = take(8 * ns);
+        result = take(8 * ns); consumed = take(8 * ns); content = take(8 * ns);
+    }
+};
+// ... and the records in d_recs, decode_dev's descriptor arrays for nc compressed and nr stored blocks, nbsum checksummed
+// ones, nf frames and nfsum content checksums, with the verdict's per-frame facts and the packing's per-block destinations.
+// They never leave the device.
+struct FrameStreamRecLayout {
+    size_t c_soff, c_doff, c_slen, c_dcap, c_res, r_soff, r_doff, r_len, k_comp, k_rawlen, k_off, k_dst, k_len;
+    size_t b_off, b_len, b_want, b_out, h_off, h_len, h_out, fr_first, fr_nblk, fr_bsum, fr_fsum, fr_size, fr_bits;
+    size_t f_first, f_nblk, f_want, f_out, bytes = 0;
+    FrameStreamRecLayout(size_t nc, size_t nr, size_t nbsum, size_t nf, size_t nfsum)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        const size_t nb = nc + nr;
+        c_soff = take(8 * nc); c_doff = take(8 * nc); c_slen = take(4 * nc); c_dcap = take(4 * nc); c_res = take(4 * nc);
+        r_soff = take(8 * nr); r_doff = take(8 * nr); r_len = take(4 * nr);
+        k_comp = take(4 * nb); k_rawlen = take(4 * nb); k_off = take(8 * nb); k_dst = take(8 * nb); k_len = take(4 * nb);
+        b_off = take(8 * nbsum); b_len = take(4 * nbsum); b_want = take(4 * nbsum); b_out = take(4 * nbsum);
+        h_off = take(8 * nf); h_len = take(4 * nf); h_out = take(4 * nf);
+        fr_first = take(4 * nf); fr_nblk = take(4 * nf); fr_bsum = take(4 * nf); fr_fsum = take(4 * nf); fr_size = take(8 * nf);
+        fr_bits = take(4 * nf);
+        f_first = take(4 * nfsum); f_nblk = take(4 * nfsum); f_want = take(4 * nfsum); f_out = take(4 * nfsum);
+    }
+};
+
+// decode_dev for many streams at once with the index built and judged on the device: counting walk, scans of the counts (only
+// their totals come to the host, to size the records and slots), recording walk, decode_dev's payload launches, one verdict
+// warp per stream, one gather into d_dst.  The launches do not depend on the number of streams, frames or blocks.
+static int frame_streams_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                        uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, bool single,
+                                        int64_t* result, uint64_t* src_consumed, uint64_t* content_len, cudaStream_t st)
+{
+    if (ns == 0) return 0;
+    if (!src_off || !src_len || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
+    if (ns > 0x7FFFFFFFull) return fail_arg("too many streams in one call");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    FrameReadScratch* s; SideStream* side;
+    int rc = get_frame_read_scratch(&s, &side);
+    const FrameStreamLayout L(ns);
+    if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
+    if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
+    if (rc) return rc;
+    uint8_t *D = s->d_seg, *H = s->h_seg;
+    memcpy(H + L.s_off, src_off, 8 * ns); memcpy(H + L.s_len, src_len, 8 * ns);
+    memcpy(H + L.d_off, dst_off, 8 * ns); memcpy(H + L.d_cap, dst_cap, 8 * ns);
+    memset(H + L.over, 0, 4);
+    FrameStreamRead r{};
+    r.src = d_src;
+    r.s_off = (const uint64_t*)(D + L.s_off); r.s_len = (const uint64_t*)(D + L.s_len);
+    r.d_off = (const uint64_t*)(D + L.d_off); r.d_cap = (const uint64_t*)(D + L.d_cap);
+    r.cnt = (int32_t*)(D + L.cnt); r.pos = (const uint64_t*)(D + L.pos);
+    r.tail = (int32_t*)(D + L.tail); r.ip = (uint64_t*)(D + L.ip); r.over = (int32_t*)(D + L.over);
+    r.result = (int64_t*)(D + L.result); r.consumed = (uint64_t*)(D + L.consumed); r.content = (uint64_t*)(D + L.content);
+    r.ns = (uint32_t)ns; r.single = single;
+    uint64_t* totals = (uint64_t*)(D + L.totals);
+
+    Drain drain{ st, side->st };
+    CK(cudaMemcpyAsync(D, H, L.totals, cudaMemcpyHostToDevice, st));
+    g_launch_count.fetch_add(1 + FS_ROWS, std::memory_order_relaxed);
+    CK(launch_frame_streams_walk(r, false, st));
+    for (int row = 0; row < FS_ROWS; row++)
+        CK(launch_scan(r.cnt + row * ns, (uint64_t*)r.pos + row * ns, totals + row, nullptr, ns, st));
+    CK(cudaMemcpyAsync(H + L.over, D + L.over, L.cnt - L.over, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint64_t* tot = (const uint64_t*)(H + L.totals);
+    const uint64_t nc = tot[FS_COMP], nr = tot[FS_RAW], nb = nc + nr, nbsum = tot[FS_BSUM], nf = tot[FS_FRAME], nfsum = tot[FS_FSUM];
+    const uint64_t slot_bytes = tot[FS_SLOT16] << 4;
+    if (*(const int32_t*)(H + L.over) || nb > 0x7FFFFFFFull || nf > 0x7FFFFFFFull)
+        return fail_arg("more than 2^31 - 1 blocks or frames in one call, or 32 GiB of decode slots in one stream");
+    const FrameStreamRecLayout R(nc, nr, nbsum, nf, nfsum);
+    rc = reserve_device(s->d_recs, s->recs_cap, R.bytes + 16);
+    if (!rc) rc = reserve_device(s->d_slots, s->slots_cap, slot_bytes + 16);
+    if (rc) return rc;
+    uint8_t *B = s->d_recs, *slots = s->d_slots;
+    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
+    r.c_slen = (int32_t*)(B + R.c_slen); r.c_dcap = (int32_t*)(B + R.c_dcap); r.c_res = (int32_t*)(B + R.c_res);
+    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
+    r.k_comp = (int32_t*)(B + R.k_comp); r.k_rawlen = (int32_t*)(B + R.k_rawlen); r.k_off = (uint64_t*)(B + R.k_off);
+    r.k_dst = (uint64_t*)(B + R.k_dst); r.k_len = (int32_t*)(B + R.k_len);
+    r.b_off = (uint64_t*)(B + R.b_off); r.b_len = (int32_t*)(B + R.b_len); r.b_want = (uint32_t*)(B + R.b_want); r.b_out = (uint32_t*)(B + R.b_out);
+    r.h_off = (uint64_t*)(B + R.h_off); r.h_len = (int32_t*)(B + R.h_len); r.h_out = (uint32_t*)(B + R.h_out);
+    r.fr_first = (uint32_t*)(B + R.fr_first); r.fr_nblk = (uint32_t*)(B + R.fr_nblk); r.fr_bsum = (int32_t*)(B + R.fr_bsum);
+    r.fr_fsum = (int32_t*)(B + R.fr_fsum); r.fr_size = (uint64_t*)(B + R.fr_size); r.fr_bits = (uint32_t*)(B + R.fr_bits);
+    r.f_first = (uint32_t*)(B + R.f_first); r.f_nblk = (uint32_t*)(B + R.f_nblk); r.f_want = (uint32_t*)(B + R.f_want); r.f_out = (uint32_t*)(B + R.f_out);
+
+    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+    CK(counted(launch_frame_streams_walk(r, true, st)));
+    if (nc) CK(cudaMemsetAsync(r.c_res, 0x80, nc * 4, st));                  // FRAME_RES_PENDING
+    // decode_dev's payload launches: descriptor and block checksums, stored blocks, then every compressed block; the content
+    // checksums follow the decoder on the side stream
+    if (nf) CK(counted(launch_xxh32(d_src, r.h_off, r.h_len, 0, r.h_out, (size_t)nf, st)));
+    if (nbsum)                      // the average stream byte per block bounds the average checksummed block
+        CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_src, r.b_off, r.b_len, 0, r.b_out, (size_t)nbsum, st)));
+    if (nr) CK(counted(launch_gather(d_src, r.r_soff, r.r_len, slots, r.r_doff, (size_t)nr, st)));
+    CK(cudaEventRecord(side->fork, st));
+    if (nc) {
+        const BatchArgs a{ d_src, r.c_soff, r.c_slen, slots, r.c_doff, r.c_dcap, r.c_res, (size_t)nc };
+        CK(counted(launch_decompress_safe(a, st)));
+    }
+    if (nfsum) {
+        CK(cudaStreamWaitEvent(side->st, side->fork, 0));
+        CK(counted(launch_xxh32_frames_chained(slots, r.k_off, r.f_first, r.f_nblk, r.k_comp, r.k_rawlen, r.c_res, r.f_out,
+                                               (size_t)nfsum, side->st)));
+        CK(cudaEventRecord(side->join, side->st));
+        CK(cudaStreamWaitEvent(st, side->join, 0));
+    }
+    // every verdict is in before anything is packed: a stream that fails writes nothing in d_dst
+    CK(counted(launch_frame_streams_verdict(r, st)));
+    if (nb) CK(counted(launch_gather(slots, r.k_off, r.k_len, d_dst, r.k_dst, (size_t)nb, st)));
+    CK(cudaMemcpyAsync(H + L.result, D + L.result, L.bytes - L.result, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    memcpy(result, H + L.result, 8 * ns);
+    if (src_consumed) memcpy(src_consumed, H + L.consumed, 8 * ns);
+    if (content_len) memcpy(content_len, H + L.content, 8 * ns);
     return 0;
 }
 
@@ -558,6 +692,15 @@ int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t n, uint8_t* d_dst, 
     CK(cudaStreamSynchronize(st));
     drain.done = true;
     return (int64_t)total;
+}
+
+// ns frame streams, each read like b200lz4f_decompress_host{,_single} would read it alone (frame_streams_decompress_dev)
+int b200lz4f_decompress_streams_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
+                                    uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int single,
+                                    int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream)
+{
+    return frame_streams_decompress_dev(d_src, src_off, src_len, ns, d_dst, dst_off, dst_cap, single != 0, result, src_consumed,
+                                        content_len, (cudaStream_t)stream);
 }
 
 } // extern "C"

@@ -164,6 +164,17 @@ __host__ __device__ inline WalkEnd walk_frames(const uint8_t* src, uint64_t n, u
     return e;
 }
 
+// The slot layout of the frame readers' decode (frame.cu's IndexSink, frame_streams.cu): a stored block needs its own size, a
+// compressed one cannot decode to more than 255 bytes per byte (one length byte adds at most 255) -- so a stream of tiny
+// flushed blocks asks for what it can fill, not for blockMaxSize each.  room is the decoder's capacity; a block takes
+// frame_slot_bytes of the layout: full blocks exactly bs, so a frame without short blocks in the middle stays contiguous,
+// the rest rounded up to 16.
+__host__ __device__ inline uint64_t frame_slot_room(uint32_t bs, uint32_t size, bool raw)
+{
+    return raw ? size : (255ull * size < bs ? 255ull * size : bs);
+}
+__host__ __device__ inline uint64_t frame_slot_bytes(uint64_t room, uint32_t bs) { return room >= bs ? bs : ((room + 15) & ~15ull); }
+
 // The device walk (frame_index.cu): one thread per segment [seg_start, seg_end) of the container, records into a region of
 // its own.  A record is 16 bytes: a frame takes two (written at frame_end into the pair reserved at frame_begin), a block one;
 // they come in stream order.  A walker whose region is full keeps counting (WalkSummary.nrec) but stops writing.
@@ -177,6 +188,34 @@ cudaError_t launch_frame_walk(const uint8_t* src, uint64_t n, bool single, const
 // walker j's lens[j] records move from recs + segs[j].rec_off to packed + pos[j]
 cudaError_t launch_frame_pack(const WalkSeg* segs, const int32_t* lens, const uint64_t* pos, const WalkRec* recs, WalkRec* packed,
                               uint32_t m, cudaStream_t st);
+
+// The device reader of many independent frame streams (frame_streams_decompress_dev in frame.cu, kernels in
+// frame_streams.cu), all device pointers.  Per stream: its bytes and room, the counting walk's counts (FS_* rows of cnt, each
+// ns entries, and their exclusive prefixes in pos), its tail code and end, and the results.  The records of every block and
+// frame, in stream order, follow decode_dev's descriptor arrays (IndexLayout in frame.cu): c_* compressed blocks (BatchArgs of
+// the safe decoder into the slots), r_* stored blocks (gather into the slots), k_* every block (the chained content checksum's
+// view, and where the verdict puts it in d_dst: k_dst / k_len), b_* checksummed blocks, h_* frame descriptors, fr_* every
+// frame, f_* frames with a content checksum.
+enum { FS_COMP, FS_RAW, FS_BSUM, FS_FRAME, FS_FSUM, FS_SLOT16, FS_ROWS };     // counts per stream; slots in 16-byte units
+struct FrameStreamRead {
+    const uint8_t* src;
+    const uint64_t *s_off, *s_len, *d_off, *d_cap;
+    int32_t* cnt; const uint64_t* pos;                                  // cnt[row * ns + s], pos likewise
+    int32_t* tail; uint64_t* ip; int32_t* over;                         // over: set when a stream's counts do not fit int32
+    int64_t* result; uint64_t *consumed, *content;
+    uint64_t *c_soff, *c_doff; int32_t *c_slen, *c_dcap, *c_res;
+    uint64_t *r_soff, *r_doff; int32_t* r_len;
+    int32_t *k_comp, *k_rawlen; uint64_t *k_off, *k_dst; int32_t* k_len;
+    uint64_t* b_off; int32_t* b_len; uint32_t *b_want, *b_out;
+    uint64_t* h_off; int32_t* h_len; uint32_t* h_out;
+    uint32_t *fr_first, *fr_nblk; int32_t *fr_bsum, *fr_fsum; uint64_t* fr_size; uint32_t* fr_bits;   // bits: hc_byte, has_size
+    uint32_t *f_first, *f_nblk, *f_want, *f_out;
+    uint32_t ns; bool single;
+};
+// one thread per stream: with `record` false the counts, tail and ip; with it every record
+cudaError_t launch_frame_streams_walk(const FrameStreamRead& r, bool record, cudaStream_t st);
+// one warp per stream: result, consumed, content, and each block's k_dst / k_len (0 for a stream that fails)
+cudaError_t launch_frame_streams_verdict(const FrameStreamRead& r, cudaStream_t st);
 
 // ---- "LZ4Block" streams (LZ4BlockOutputStream.java:203-266, LZ4BlockInputStream.java:191-264).  The writer is the frame
 // writer's loop (compress_blocks_dev in containers.cu) with lz4block.cu's item sizes, emit and seal: the same FramePlan, a

@@ -136,6 +136,33 @@ def decompress_frames_dev(src, max_decoded: int, read_single_frame: bool = False
     return out[:r]
 
 
+def decompress_frame_streams_dev(src, src_off, src_len, out, dst_off, dst_cap, read_single_frame: bool = False):
+    """many independent LZ4 frame streams in device memory, each read as its own LZ4FrameInputStream(in, readSingleFrame) into
+    device memory (b200lz4f_decompress_streams_dev): stream s is src[src_off[s] : src_off[s] + src_len[s]], decoded to
+    out[dst_off[s]:] with room for dst_cap[s] bytes.  No byte of the streams or the content crosses to the host.  src, out:
+    contiguous uint8 CUDA tensors on one device; the offsets and lengths: host sequences.  Runs on torch's current stream and
+    returns when the results are on the host.  -> (result, src_consumed, content_len), np.int64 / np.uint64 / np.uint64
+    arrays: per stream what decompress_frames would return (decoded bytes, or the LZ4FrameError code -1 .. -10), where the
+    reader stopped (0 on an error), and what it decodes to when room is not the limit.  Raises only on a backend error."""
+    import torch
+    off, ln = _dev_streams(src, src_off, src_len, "stream")
+    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+    if len(doff) != len(ln) or len(dcap) != len(ln):
+        raise ValueError("dst_off and dst_cap must have one entry per stream")
+    if len(ln) and int((doff + dcap).max()) > out.numel():
+        raise ValueError("a destination range reaches past the end of out")
+    result = np.zeros(len(ln), dtype=np.int64)
+    consumed, content = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
+    N.check(N.lib().b200lz4f_decompress_streams_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
+                                                    doff.ctypes.data, dcap.ctypes.data, int(bool(read_single_frame)),
+                                                    result.ctypes.data, consumed.ctypes.data, content.ctypes.data,
+                                                    torch.cuda.current_stream(src.device).cuda_stream))
+    return result, consumed, content
+
+
 # ---- lz4-java's private "LZ4Block" container (LZ4BlockOutputStream / LZ4BlockInputStream)
 def compress_lz4block(src, block_size: int = 1 << 16, hc_level: int = 0) -> bytes:
     s = _view(src)
