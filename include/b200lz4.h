@@ -274,6 +274,48 @@ int64_t b200lz4f_decompress_dev(const uint8_t* d_src, size_t srcSize, uint8_t* d
 int     b200lz4f_decompress_streams_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
                                         uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int single,
                                         int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream);
+/* Incremental device-resident LZ4 Frame reader for ns streams, each one LZ4FrameInputStream(in, readSingleFrame) whose bytes
+ * arrive in pieces: the incremental counterpart of b200lz4f_decompress_streams_dev, built from the same parts.  A reader
+ * (b200lz4f_reader_create, ns above 2^31 - 1: NULL with *err = B200LZ4_E_ARG) is host data, about 80 bytes of state per
+ * stream; create and free make no CUDA call.  Any thread may use a reader, one at a time (it is not thread-safe, like
+ * LZ4FrameInputStream).
+ * b200lz4f_reader_read_dev: stream s's next piece is src_len[s] bytes at d_src + src_off[s]; its content goes to d_dst +
+ * dst_off[s] with room dst_cap[s]; eof[s] != 0 says the piece ends the stream (HOST arrays of ns entries; the bytes device
+ * memory of the current device).  Per stream:
+ *  - The call takes the complete units at the start of the piece, in stream order, and stops in front of the first
+ *    incomplete one.  A unit is a frame header (magic to HC byte), a block (word, payload and block checksum), the EndMark with
+ *    its content checksum, or a skippable frame's 8-byte header; a skippable frame's payload is taken in any portions.
+ *    src_consumed[s] is where it stopped: the next piece must start at that byte of the stream.  The reader keeps no payload
+ *    byte between calls.
+ *  - The content is packed into [dst_off[s], dst_off[s] + produced[s]).  A block is taken only while the room left holds its
+ *    slot bound (a stored block its size, a compressed one min(blockMaxSize, 255 * its size)), so nothing is written outside
+ *    that range and there is no -9.  With dst_cap[s] >= the frame's blockMaxSize every call with a complete unit progresses.
+ *  - status[s]: B200LZ4F_MORE_INPUT (need[s] = the bytes from src_consumed the next unit takes, or those that make its length
+ *    readable), B200LZ4F_MORE_ROOM (the first block the call could take does not fit; need[s] = its slot bound),
+ *    B200LZ4F_DONE (the stream ended on a frame boundary with eof, or with single != 0 behind the first non-skippable frame),
+ *    or -1 .. -10 as for b200lz4f_decompress_host: an incomplete unit with eof is -1, and a stream with no frame at all is
+ *    what the host reader gives it.  Errors come in stream order: the blocks in front of the failing unit are delivered and
+ *    counted in produced[s] (what LZ4FrameInputStream returns before it throws), the failing block writes nothing, and a -7
+ *    or -8 comes after the frame's whole content; src_consumed[s] is where the failing unit starts.  DONE and every error
+ *    are latched: later calls return the same status and take and produce nothing.
+ *  - Whatever the pieces and room, the concatenated content and the final status are what b200lz4f_decompress_host /
+ *    _single returns for the whole stream, with the same total src_consumed.  The content checksum (four lanes, an open
+ *    stripe, a 64-bit length) and the content count travel in the state, so frames above 4 GiB are checked.
+ * Returns 0 or B200LZ4_E_*: a NULL reader or pointer, ns other than the reader's, or a destination range that overflows are
+ * found before anything is launched; more than 2^31 - 1 blocks or frames in one call after the first walk.  The number of
+ * launches does not depend on ns or on the number of frames or blocks; two synchronisations (scan totals, end); only the
+ * per-stream arguments, states and results and a few totals cross to and from the host, no block record and no payload
+ * byte.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep scratch
+ * of the thread's context (the frame reader's segment buffers, record regions and decode slots), sized by the call -- the
+ * pieces, the blocks taken, the room -- never by how long a stream has been read. */
+#define B200LZ4F_MORE_INPUT 0
+#define B200LZ4F_MORE_ROOM  1
+#define B200LZ4F_DONE       2
+void*   b200lz4f_reader_create(size_t ns, int single, int* err);
+int     b200lz4f_reader_read_dev(void* reader, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                 const uint8_t* eof, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                 int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream);
+void    b200lz4f_reader_free(void* reader);
 /* Device-resident LZ4 Frame writer (LZ4FrameOutputStream.java:178-251) for nf independent frames, with bsCode / flags /
  * hc_level as b200lz4f_compress_host_hc takes them.  Frame f is src_len[f] bytes at d_src + src_off[f] (src_off / src_len:
  * HOST arrays of nf entries; the bytes are in device memory of the current device).  The frames are written back to back

@@ -76,6 +76,9 @@ SYMBOLS = [
     ("b200lz4f_index_create_dev", _vp, [_vp, _sz, _i, _vp, _sz, _vp, _vp, _vp, _vp]),
     ("b200lz4f_decompress_dev", C.c_int64, [_vp, _sz, _vp, _sz, _i, _vp, _sz, _vp, _vp]),
     ("b200lz4f_decompress_streams_dev", _i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    ("b200lz4f_reader_create", _vp, [_sz, _i, _vp]),
+    ("b200lz4f_reader_read_dev", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    ("b200lz4f_reader_free", None, [_vp]),
     ("b200lz4f_compress_dev", C.c_int64, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _i, _i, _i, _vp]),
     ("b200lz4f_compress_bound", _sz, [_sz, _i]),
     ("b200lz4f_compress_host", C.c_int64, [_vp, _sz, _vp, _sz, _i, _i]),

@@ -20,6 +20,7 @@
 #ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device readers' kernels come with it
 #include "frame_index.cu"
 #include "frame_streams.cu"
+#include "frame_reader.cu"
 #endif
 #include <algorithm>
 #include <cstring>
@@ -338,6 +339,53 @@ struct FrameStreamRecLayout {
     }
 };
 
+// Points r's record arrays into the call's record region B.
+static void bind_stream_records(FrameStreamRead& r, uint8_t* B, const FrameStreamRecLayout& R)
+{
+    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
+    r.c_slen = (int32_t*)(B + R.c_slen); r.c_dcap = (int32_t*)(B + R.c_dcap); r.c_res = (int32_t*)(B + R.c_res);
+    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
+    r.k_comp = (int32_t*)(B + R.k_comp); r.k_rawlen = (int32_t*)(B + R.k_rawlen); r.k_off = (uint64_t*)(B + R.k_off);
+    r.k_dst = (uint64_t*)(B + R.k_dst); r.k_len = (int32_t*)(B + R.k_len);
+    r.b_off = (uint64_t*)(B + R.b_off); r.b_len = (int32_t*)(B + R.b_len); r.b_want = (uint32_t*)(B + R.b_want); r.b_out = (uint32_t*)(B + R.b_out);
+    r.h_off = (uint64_t*)(B + R.h_off); r.h_len = (int32_t*)(B + R.h_len); r.h_out = (uint32_t*)(B + R.h_out);
+    r.fr_first = (uint32_t*)(B + R.fr_first); r.fr_nblk = (uint32_t*)(B + R.fr_nblk); r.fr_bsum = (int32_t*)(B + R.fr_bsum);
+    r.fr_fsum = (int32_t*)(B + R.fr_fsum); r.fr_size = (uint64_t*)(B + R.fr_size); r.fr_bits = (uint32_t*)(B + R.fr_bits);
+    r.f_first = (uint32_t*)(B + R.f_first); r.f_nblk = (uint32_t*)(B + R.f_nblk); r.f_want = (uint32_t*)(B + R.f_want); r.f_out = (uint32_t*)(B + R.f_out);
+}
+
+// decode_dev's payload launches behind a recording walk: descriptor and block checksums, stored blocks, then every compressed
+// block; the content checksums follow the decoder on the side stream (with carry / mode: launch_xxh32_frames_chained_carry).
+static int stream_payload_launches(const FrameStreamRead& r, uint8_t* slots, uint64_t bytes, uint64_t nc, uint64_t nr,
+                                   uint64_t nbsum, uint64_t nf, uint64_t nfsum, SideStream* side, cudaStream_t st,
+                                   Xxh32Carry* carry = nullptr, const uint8_t* mode = nullptr)
+{
+    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+    const uint64_t nb = nc + nr;
+    if (nc) CK(cudaMemsetAsync(r.c_res, 0x80, nc * 4, st));                  // FRAME_RES_PENDING
+    if (nf) CK(counted(launch_xxh32(r.src, r.h_off, r.h_len, 0, r.h_out, (size_t)nf, st)));
+    if (nbsum)                      // the average stream byte per block bounds the average checksummed block
+        CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(r.src, r.b_off, r.b_len, 0, r.b_out, (size_t)nbsum, st)));
+    if (nr) CK(counted(launch_gather(r.src, r.r_soff, r.r_len, slots, r.r_doff, (size_t)nr, st)));
+    CK(cudaEventRecord(side->fork, st));
+    if (nc) {
+        const BatchArgs a{ r.src, r.c_soff, r.c_slen, slots, r.c_doff, r.c_dcap, r.c_res, (size_t)nc };
+        CK(counted(launch_decompress_safe(a, st)));
+    }
+    if (nfsum) {
+        CK(cudaStreamWaitEvent(side->st, side->fork, 0));
+        if (carry)
+            CK(counted(launch_xxh32_frames_chained_carry(slots, r.k_off, r.f_first, r.f_nblk, r.k_comp, r.k_rawlen, r.c_res, r.f_out,
+                                                         (size_t)nfsum, carry, mode, side->st)));
+        else
+            CK(counted(launch_xxh32_frames_chained(slots, r.k_off, r.f_first, r.f_nblk, r.k_comp, r.k_rawlen, r.c_res, r.f_out,
+                                                   (size_t)nfsum, side->st)));
+        CK(cudaEventRecord(side->join, side->st));
+        CK(cudaStreamWaitEvent(st, side->join, 0));
+    }
+    return 0;
+}
+
 // decode_dev for many streams at once with the index built and judged on the device: counting walk, scans of the counts (only
 // their totals come to the host, to size the records and slots), recording walk, decode_dev's payload launches, one verdict
 // warp per stream, one gather into d_dst.  The launches do not depend on the number of streams, frames or blocks.
@@ -392,39 +440,13 @@ static int frame_streams_decompress_dev(const uint8_t* d_src, const uint64_t* sr
     rc = reserve_device(s->d_recs, s->recs_cap, R.bytes + 16);
     if (!rc) rc = reserve_device(s->d_slots, s->slots_cap, slot_bytes + 16);
     if (rc) return rc;
-    uint8_t *B = s->d_recs, *slots = s->d_slots;
-    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
-    r.c_slen = (int32_t*)(B + R.c_slen); r.c_dcap = (int32_t*)(B + R.c_dcap); r.c_res = (int32_t*)(B + R.c_res);
-    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
-    r.k_comp = (int32_t*)(B + R.k_comp); r.k_rawlen = (int32_t*)(B + R.k_rawlen); r.k_off = (uint64_t*)(B + R.k_off);
-    r.k_dst = (uint64_t*)(B + R.k_dst); r.k_len = (int32_t*)(B + R.k_len);
-    r.b_off = (uint64_t*)(B + R.b_off); r.b_len = (int32_t*)(B + R.b_len); r.b_want = (uint32_t*)(B + R.b_want); r.b_out = (uint32_t*)(B + R.b_out);
-    r.h_off = (uint64_t*)(B + R.h_off); r.h_len = (int32_t*)(B + R.h_len); r.h_out = (uint32_t*)(B + R.h_out);
-    r.fr_first = (uint32_t*)(B + R.fr_first); r.fr_nblk = (uint32_t*)(B + R.fr_nblk); r.fr_bsum = (int32_t*)(B + R.fr_bsum);
-    r.fr_fsum = (int32_t*)(B + R.fr_fsum); r.fr_size = (uint64_t*)(B + R.fr_size); r.fr_bits = (uint32_t*)(B + R.fr_bits);
-    r.f_first = (uint32_t*)(B + R.f_first); r.f_nblk = (uint32_t*)(B + R.f_nblk); r.f_want = (uint32_t*)(B + R.f_want); r.f_out = (uint32_t*)(B + R.f_out);
+    uint8_t* slots = s->d_slots;
+    bind_stream_records(r, s->d_recs, R);
 
     auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     CK(counted(launch_frame_streams_walk(r, true, st)));
-    if (nc) CK(cudaMemsetAsync(r.c_res, 0x80, nc * 4, st));                  // FRAME_RES_PENDING
-    // decode_dev's payload launches: descriptor and block checksums, stored blocks, then every compressed block; the content
-    // checksums follow the decoder on the side stream
-    if (nf) CK(counted(launch_xxh32(d_src, r.h_off, r.h_len, 0, r.h_out, (size_t)nf, st)));
-    if (nbsum)                      // the average stream byte per block bounds the average checksummed block
-        CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_src, r.b_off, r.b_len, 0, r.b_out, (size_t)nbsum, st)));
-    if (nr) CK(counted(launch_gather(d_src, r.r_soff, r.r_len, slots, r.r_doff, (size_t)nr, st)));
-    CK(cudaEventRecord(side->fork, st));
-    if (nc) {
-        const BatchArgs a{ d_src, r.c_soff, r.c_slen, slots, r.c_doff, r.c_dcap, r.c_res, (size_t)nc };
-        CK(counted(launch_decompress_safe(a, st)));
-    }
-    if (nfsum) {
-        CK(cudaStreamWaitEvent(side->st, side->fork, 0));
-        CK(counted(launch_xxh32_frames_chained(slots, r.k_off, r.f_first, r.f_nblk, r.k_comp, r.k_rawlen, r.c_res, r.f_out,
-                                               (size_t)nfsum, side->st)));
-        CK(cudaEventRecord(side->join, side->st));
-        CK(cudaStreamWaitEvent(st, side->join, 0));
-    }
+    rc = stream_payload_launches(r, slots, bytes, nc, nr, nbsum, nf, nfsum, side, st);
+    if (rc) return rc;
     // every verdict is in before anything is packed: a stream that fails writes nothing in d_dst
     CK(counted(launch_frame_streams_verdict(r, st)));
     if (nb) CK(counted(launch_gather(slots, r.k_off, r.k_len, d_dst, r.k_dst, (size_t)nb, st)));
@@ -434,6 +456,114 @@ static int frame_streams_decompress_dev(const uint8_t* d_src, const uint64_t* sr
     memcpy(result, H + L.result, 8 * ns);
     if (src_consumed) memcpy(src_consumed, H + L.consumed, 8 * ns);
     if (content_len) memcpy(content_len, H + L.content, 8 * ns);
+    return 0;
+}
+
+// ---- the incremental reader (b200lz4f_reader_*; kernels: frame_reader.cu).  The reader is host data: one state per stream.
+struct FrameReaderHandle {
+    size_t ns; bool single;
+    std::vector<FrameReaderState> st;
+};
+// One call's per-stream arrays in d_seg / h_seg: the arguments, the states and the zeroed `over` word go up; `over` and the
+// scan totals come back after the counting walk, the results and the new states at the end.
+struct FrameReaderLayout {
+    size_t s_off, s_len, d_off, d_cap, eof, st_in, over, totals, cnt, pos, tail, status, consumed, produced, need, st_out, bytes = 0;
+    explicit FrameReaderLayout(size_t ns)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        s_off = take(8 * ns); s_len = take(8 * ns); d_off = take(8 * ns); d_cap = take(8 * ns); eof = take(ns);
+        st_in = take(sizeof(FrameReaderState) * ns);
+        over = take(4); totals = take(8 * FS_ROWS);
+        cnt = take(4 * FS_ROWS * ns); pos = take(8 * FS_ROWS * ns); tail = take(4 * ns);
+        status = take(4 * ns); consumed = take(8 * ns); produced = take(8 * ns); need = take(8 * ns);
+        st_out = take(sizeof(FrameReaderState) * ns);
+    }
+};
+
+// frame_streams_decompress_dev's steps from each stream's carried state: counting walk, scans (their totals come to the
+// host), recording walk, decode_dev's payload launches with the carried content checksums, one verdict warp per stream,
+// one gather of the blocks in front of each stream's cut.
+static int frame_reader_read_dev(FrameReaderHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                 const uint8_t* eof, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                 int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
+{
+    if (!h) return fail_arg("null reader");
+    const size_t ns = h->ns;
+    if (ns == 0) return 0;
+    if (!src_off || !src_len || !eof || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
+        return fail_arg("null pointer");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    FrameReadScratch* s; SideStream* side;
+    int rc = get_frame_read_scratch(&s, &side);
+    const FrameReaderLayout L(ns);
+    if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
+    if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
+    if (rc) return rc;
+    uint8_t *D = s->d_seg, *H = s->h_seg;
+    memcpy(H + L.s_off, src_off, 8 * ns); memcpy(H + L.s_len, src_len, 8 * ns);
+    memcpy(H + L.d_off, dst_off, 8 * ns); memcpy(H + L.d_cap, dst_cap, 8 * ns); memcpy(H + L.eof, eof, ns);
+    memcpy(H + L.st_in, h->st.data(), sizeof(FrameReaderState) * ns);
+    memset(H + L.over, 0, 4);
+    FrameReaderRead q{};
+    FrameStreamRead& r = q.r;
+    r.src = d_src;
+    r.s_off = (const uint64_t*)(D + L.s_off); r.s_len = (const uint64_t*)(D + L.s_len);
+    r.d_off = (const uint64_t*)(D + L.d_off); r.d_cap = (const uint64_t*)(D + L.d_cap);
+    r.cnt = (int32_t*)(D + L.cnt); r.pos = (const uint64_t*)(D + L.pos);
+    r.tail = (int32_t*)(D + L.tail); r.over = (int32_t*)(D + L.over); r.consumed = (uint64_t*)(D + L.consumed);
+    r.ns = (uint32_t)ns; r.single = h->single;
+    q.eof = D + L.eof;
+    q.st_in = (const FrameReaderState*)(D + L.st_in); q.st_out = (FrameReaderState*)(D + L.st_out);
+    q.status = (int32_t*)(D + L.status); q.produced = (uint64_t*)(D + L.produced); q.need = (uint64_t*)(D + L.need);
+    uint64_t* totals = (uint64_t*)(D + L.totals);
+
+    Drain drain{ st, side->st };
+    CK(cudaMemcpyAsync(D, H, L.totals, cudaMemcpyHostToDevice, st));
+    g_launch_count.fetch_add(1 + FS_ROWS, std::memory_order_relaxed);
+    CK(launch_frame_reader_walk(q, false, st));
+    for (int row = 0; row < FS_ROWS; row++)
+        CK(launch_scan(r.cnt + row * ns, (uint64_t*)r.pos + row * ns, totals + row, nullptr, ns, st));
+    CK(cudaMemcpyAsync(H + L.over, D + L.over, L.cnt - L.over, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint64_t* tot = (const uint64_t*)(H + L.totals);
+    const uint64_t nc = tot[FS_COMP], nr = tot[FS_RAW], nb = nc + nr, nbsum = tot[FS_BSUM], nf = tot[FS_FRAME], nfsum = tot[FS_FSUM];
+    const uint64_t slot_bytes = tot[FS_SLOT16] << 4;
+    if (*(const int32_t*)(H + L.over) || nb > 0x7FFFFFFFull || nf > 0x7FFFFFFFull)
+        return fail_arg("more than 2^31 - 1 blocks or frames in one call, or 32 GiB of decode slots in one stream");
+    // decode_dev's records, then the reader's own: unit starts, frame parts, carried content checksums
+    const FrameStreamRecLayout R(nc, nr, nbsum, nf, nfsum);
+    size_t x = R.bytes;
+    auto take = [&](size_t n) { const size_t at = x; x = (x + n + 15) & ~size_t(15); return at; };
+    const size_t k_at = take(8 * nb), fr_at = take(8 * nf), fr_end_at = take(8 * nf), fr_mode = take(4 * nf);
+    const size_t f_carry = take(sizeof(Xxh32Carry) * nfsum), f_mode = take(nfsum);
+    rc = reserve_device(s->d_recs, s->recs_cap, x + 16);
+    if (!rc) rc = reserve_device(s->d_slots, s->slots_cap, slot_bytes + 16);
+    if (rc) return rc;
+    uint8_t *B = s->d_recs, *slots = s->d_slots;
+    bind_stream_records(r, B, R);
+    q.k_at = (uint64_t*)(B + k_at); q.fr_at = (uint64_t*)(B + fr_at); q.fr_end_at = (uint64_t*)(B + fr_end_at);
+    q.fr_mode = (uint32_t*)(B + fr_mode); q.f_carry = (Xxh32Carry*)(B + f_carry); q.f_mode = B + f_mode;
+
+    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+    CK(counted(launch_frame_reader_walk(q, true, st)));
+    rc = stream_payload_launches(r, slots, bytes, nc, nr, nbsum, nf, nfsum, side, st, q.f_carry, q.f_mode);
+    if (rc) return rc;
+    CK(counted(launch_frame_reader_verdict(q, st)));
+    if (nb) CK(counted(launch_gather(slots, r.k_off, r.k_len, d_dst, r.k_dst, (size_t)nb, st)));
+    CK(cudaMemcpyAsync(H + L.status, D + L.status, L.bytes - L.status, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    memcpy(status, H + L.status, 4 * ns);
+    memcpy(src_consumed, H + L.consumed, 8 * ns);
+    memcpy(produced, H + L.produced, 8 * ns);
+    memcpy(need, H + L.need, 8 * ns);
+    memcpy(h->st.data(), H + L.st_out, sizeof(FrameReaderState) * ns);
     return 0;
 }
 
@@ -702,5 +832,28 @@ int b200lz4f_decompress_streams_dev(const uint8_t* d_src, const uint64_t* src_of
     return frame_streams_decompress_dev(d_src, src_off, src_len, ns, d_dst, dst_off, dst_cap, single != 0, result, src_consumed,
                                         content_len, (cudaStream_t)stream);
 }
+
+// the incremental reader (frame_reader_read_dev): host data only, no CUDA call in create or free
+void* b200lz4f_reader_create(size_t ns, int single, int* err)
+{
+    if (err) *err = 0;
+    if (ns > 0x7FFFFFFFull) { const int rc = fail_arg("too many streams in one reader"); if (err) *err = rc; return nullptr; }
+    FrameReaderHandle* h = new (std::nothrow) FrameReaderHandle;
+    if (!h) { const int rc = fail_arg("out of host memory"); if (err) *err = rc; return nullptr; }
+    h->ns = ns; h->single = single != 0;
+    try { h->st.assign(ns, FrameReaderState{}); }
+    catch (...) { delete h; const int rc = fail_arg("out of host memory"); if (err) *err = rc; return nullptr; }
+    return h;
+}
+
+int b200lz4f_reader_read_dev(void* reader, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                             const uint8_t* eof, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                             int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream)
+{
+    return frame_reader_read_dev((FrameReaderHandle*)reader, d_src, src_off, src_len, eof, d_dst, dst_off, dst_cap, status,
+                                 src_consumed, produced, need, (cudaStream_t)stream);
+}
+
+void b200lz4f_reader_free(void* reader) { delete (FrameReaderHandle*)reader; }
 
 } // extern "C"

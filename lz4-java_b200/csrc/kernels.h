@@ -34,9 +34,19 @@ cudaError_t launch_xxh32_long(const uint8_t* base, const uint64_t* off, const in
                               uint32_t* out, size_t n, cudaStream_t st);
 // frame content checksums chained to the block decoder (frame.cu): one warp per frame follows the decoder's result words
 static constexpr int32_t FRAME_RES_PENDING = int32_t(0x80808080);      // what cudaMemset(0x80) leaves; no decoder result looks like it
+// A content checksum carried from call to call (the incremental reader, frame_reader.cu): XXH32's four lanes, the bytes of
+// an unfinished stripe and the length so far.
+struct Xxh32Carry { uint64_t total; uint32_t v[4]; uint8_t mem[16]; uint32_t memsize, pad; };
+enum { XXH_CARRY_IN = 1, XXH_CARRY_OUT = 2 };   // mode[f]: start from carry[f]; leave the state in carry[f] instead of out[f]
+// every frame starts fresh and ends in its digest
 cudaError_t launch_xxh32_frames_chained(const uint8_t* slots, const uint64_t* blk_off, const uint32_t* f_first, const uint32_t* f_nblk,
                                         const int32_t* blk_comp, const int32_t* blk_rawlen, const int32_t* c_res,
                                         uint32_t* out, size_t n, cudaStream_t st);
+// the same with a carried state per frame (mode: XXH_CARRY_* per frame); one launcher for both builds (B200_LAUNCH)
+cudaError_t launch_xxh32_frames_chained_carry(const uint8_t* slots, const uint64_t* blk_off, const uint32_t* f_first,
+                                              const uint32_t* f_nblk, const int32_t* blk_comp, const int32_t* blk_rawlen,
+                                              const int32_t* c_res, uint32_t* out, size_t n, Xxh32Carry* carry,
+                                              const uint8_t* mode, cudaStream_t st);
 cudaError_t launch_xxh64(const uint8_t* base, const uint64_t* off, const int32_t* len, uint64_t seed,
                          uint64_t* out, size_t n, cudaStream_t st);
 
@@ -97,7 +107,15 @@ struct WalkFrame {
     uint8_t flg, bd, hc_byte, desc_len;
     bool complete, has_checksum, has_size;   // read up to its EndMark (and content checksum); the content checks that apply
 };
-struct WalkEnd { uint64_t ip; int err; bool seen, single_done; };   // where it stopped and why; seen: any frame, skippable ones too
+// Where it stopped and why; seen: any frame, skippable ones too.  A resumable walk (more input may come, or room is limited)
+// may also stop in front of a unit: stop says why, at where that unit starts, need what it takes (see walk_frames_from).
+struct WalkEnd { uint64_t ip; int err; bool seen, single_done; uint8_t stop; uint64_t at, need; };
+enum { WALK_STOP_NONE = 0, WALK_STOP_INPUT = 1, WALK_STOP_ROOM = 2 };
+// Where a walk starts, and where a resumable one stopped: between frames, inside a frame's blocks (that frame's FLG and BD),
+// or inside a skippable frame's payload with `skip` bytes to go.  seen: any frame so far.  A fresh WalkPos is the start of
+// a stream.
+enum { WALK_AT_FRAME = 0, WALK_IN_BLOCKS = 1, WALK_IN_SKIP = 2 };
+struct WalkPos { uint64_t skip; uint8_t where, flg, bd; bool seen; };
 
 // Walks the frames of src[0, n) from ip, which must be where a frame (or a skippable frame) starts.  Stops at the first frame
 // boundary at or past stop_at, at the end of src, at the first malformed spot (err, -1 -2 -4 -10) or, with `single`, behind
@@ -105,63 +123,112 @@ struct WalkEnd { uint64_t ip; int err; bool seen, single_done; };   // where it 
 // block(src_off, word, checksum) per complete block, and frame_end -- also for a frame the container breaks off inside
 // (complete = false).  Whether an error is the container's or the reader's is the caller's to say (it depends on what came
 // before ip).
+//
+// walk_frames_from is the same walk, resumable (the incremental reader, frame_reader.cu).  It starts at `pos`, which it
+// leaves where it stopped.  A unit is a frame header (magic to HC byte), a block (word, payload and block checksum), the
+// EndMark with its content checksum, or a skippable frame's 8-byte header; a skippable frame's payload is taken in any
+// portions.  With `more` (bytes past n may come) a unit that src holds only in part is not an error: the walk stops in front
+// of it (WALK_STOP_INPUT, need = the unit's length once that is readable, else the bytes that make it readable).  A block
+// whose slot room (frame_slot_room) is above `room` stops it in front of that block (WALK_STOP_ROOM, need = that room);
+// `room` is debited by each block taken.  A frame the walk enters inside its blocks gets frame_begin with desc_len 0 (no
+// header in src) and only flg and bd set.  With a fresh pos, `more` false and room above 4 MiB it is walk_frames exactly.
+__host__ __device__ inline uint64_t frame_slot_room(uint32_t bs, uint32_t size, bool raw);
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Sink>
+__host__ __device__ inline WalkEnd walk_frames_from(const uint8_t* src, uint64_t n, uint64_t ip, uint64_t stop_at, bool single,
+                                                    WalkPos& pos, bool more, uint64_t room, Sink& sink)
+{
+    WalkEnd e{ ip, 0, pos.seen, false, WALK_STOP_NONE, ip, 0 };
+    uint64_t unit = ip;                                                         // where the unit being read starts
+    // src ends inside the unit at `unit`, which takes `len` bytes: more may come, or the stream is cut short
+#define WALK_SHORT(len) do { if (more) { e.stop = WALK_STOP_INPUT; e.need = (len); ip = unit; } else e.err = -1; } while (0)
+    bool in_blocks = pos.where == WALK_IN_BLOCKS;
+    if (pos.where == WALK_IN_SKIP) {                                            // the rest of a skippable payload
+        const uint64_t t = pos.skip < n - ip ? pos.skip : n - ip;
+        ip += t; pos.skip -= t; unit = ip;
+        if (pos.skip) { if (more) { e.stop = WALK_STOP_INPUT; e.need = pos.skip; } else e.err = -1; }
+        else { pos.where = WALK_AT_FRAME; e.seen = true; }
+    }
+    while (!e.err && !e.stop && (in_blocks || (ip < n && ip < stop_at))) {
+        WalkFrame f{};
+        if (in_blocks) {                                                        // a frame the walk enters inside its blocks
+            f.flg = pos.flg; f.bd = pos.bd; f.has_size = f.flg & 8; in_blocks = false; pos.where = WALK_AT_FRAME;
+        } else {
+            unit = ip;
+            if (n - ip < 4) { WALK_SHORT(4); break; }
+            const uint32_t magic = rd32(src + ip); ip += 4;
+            if ((magic >> 4) == (0x184D2A50u >> 4)) {                           // skippable (:154,162-173)
+                if (n - ip < 4) { WALK_SHORT(8); break; }
+                const uint32_t sz = rd32(src + ip); ip += 4;
+                if (n - ip < sz) {
+                    if (!more) { e.err = -1; break; }
+                    pos.where = WALK_IN_SKIP; pos.skip = sz - (n - ip); ip = unit = n;
+                    e.stop = WALK_STOP_INPUT; e.need = pos.skip; break;
+                }
+                ip += sz; e.seen = true; continue;
+            }
+            if (magic != 0x184D2204u) { e.err = -2; break; }                    // (:151)
+            f.desc_off = ip;
+            if (n - ip < 3) { WALK_SHORT(n - ip ? 7 + ((src[ip] & 8) ? 8 : 0) : 5); break; }
+            f.flg = src[ip++]; f.bd = src[ip++];
+            if ((f.flg >> 6) != 1 || (f.flg & 2) || !(f.flg & 0x20) || (f.flg & 1)) { e.err = -10; break; }   // version, reserved, B.Indep, dictID
+            if ((f.bd & 0x8F) || (f.bd >> 4) < 4) { e.err = -10; break; }
+            f.has_size = f.flg & 8;
+            if (f.has_size) { if (n - ip < 9) { WALK_SHORT(15); break; } f.content_size = (uint64_t)rd32(src + ip) | ((uint64_t)rd32(src + ip + 4) << 32); ip += 8; }
+            if (n - ip < 1) { WALK_SHORT(7); break; }
+            f.desc_len = (uint8_t)(ip - f.desc_off);
+            f.hc_byte = src[ip++];
+        }
+        const uint32_t bs = 1u << (8 + 2 * (f.bd >> 4));
+        sink.frame_begin(f);
+        for (;;) {                                                              // readBlock (:258-321)
+            unit = ip;
+            if (n - ip < 4) { WALK_SHORT(4); break; }
+            const uint32_t word = rd32(src + ip); ip += 4;
+            const uint32_t sz = word & 0x7FFFFFFFu;
+            if (sz == 0) break;                                                 // EndMark
+            if (sz > bs) { e.err = -4; break; }
+            const uint64_t at = ip, len = 4ull + sz + ((f.flg & 0x10) ? 4 : 0);
+            if (n - ip < sz) { WALK_SHORT(len); break; }
+            ip += sz;
+            uint32_t sum = 0;
+            if (f.flg & 0x10) { if (n - ip < 4) { WALK_SHORT(len); break; } sum = rd32(src + ip); ip += 4; }
+            const uint64_t need = frame_slot_room(bs, sz, word >> 31);
+            if (need > room) { e.stop = WALK_STOP_ROOM; e.need = need; ip = unit; break; }
+            room -= need;
+            sink.block(at, word, sum);
+            f.nblocks++;
+        }
+        f.complete = !e.err && !e.stop;
+        f.has_checksum = f.complete && (f.flg & 4);
+        if (f.has_checksum) {
+            if (n - ip < 4) { WALK_SHORT(8); f.complete = false; f.has_checksum = false; }
+            else { f.content_checksum = rd32(src + ip); ip += 4; }
+        }
+        if (!f.complete) f.has_size = false;
+        sink.frame_end(f); e.seen = true;
+        if (e.stop) { pos.where = WALK_IN_BLOCKS; pos.flg = f.flg; pos.bd = f.bd; break; }
+        if (single) { e.single_done = true; break; }                           // readSingleFrame (:83-91, 327, 346): the rest is not read
+        if (e.err) break;
+    }
+#undef WALK_SHORT
+    if (more && !e.err && !e.stop && !e.single_done && ip >= n) { e.stop = WALK_STOP_INPUT; e.need = 4; unit = ip; }
+    pos.seen = e.seen;
+    e.ip = ip;
+    e.at = (e.err || e.stop) ? unit : ip;
+    return e;
+}
+
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
 template <class Sink>
 __host__ __device__ inline WalkEnd walk_frames(const uint8_t* src, uint64_t n, uint64_t ip, uint64_t stop_at, bool single, Sink& sink)
 {
-    WalkEnd e{ ip, 0, false, false };
-    while (ip < n && ip < stop_at) {
-        if (n - ip < 4) { e.err = -1; break; }
-        const uint32_t magic = rd32(src + ip); ip += 4;
-        if ((magic >> 4) == (0x184D2A50u >> 4)) {                               // skippable (:154,162-173)
-            if (n - ip < 4) { e.err = -1; break; }
-            const uint32_t sz = rd32(src + ip); ip += 4;
-            if (n - ip < sz) { e.err = -1; break; }
-            ip += sz; e.seen = true; continue;
-        }
-        if (magic != 0x184D2204u) { e.err = -2; break; }                        // (:151)
-        WalkFrame f{};
-        f.desc_off = ip;
-        if (n - ip < 3) { e.err = -1; break; }
-        f.flg = src[ip++]; f.bd = src[ip++];
-        if ((f.flg >> 6) != 1 || (f.flg & 2) || !(f.flg & 0x20) || (f.flg & 1)) { e.err = -10; break; }   // version, reserved, B.Indep, dictID
-        if ((f.bd & 0x8F) || (f.bd >> 4) < 4) { e.err = -10; break; }
-        const uint32_t bs = 1u << (8 + 2 * (f.bd >> 4));
-        f.has_size = f.flg & 8;
-        if (f.has_size) { if (n - ip < 9) { e.err = -1; break; } f.content_size = (uint64_t)rd32(src + ip) | ((uint64_t)rd32(src + ip + 4) << 32); ip += 8; }
-        if (n - ip < 1) { e.err = -1; break; }
-        f.desc_len = (uint8_t)(ip - f.desc_off);
-        f.hc_byte = src[ip++];
-        sink.frame_begin(f);
-        for (;;) {                                                              // readBlock (:258-321)
-            if (n - ip < 4) { e.err = -1; break; }
-            const uint32_t word = rd32(src + ip); ip += 4;
-            const uint32_t sz = word & 0x7FFFFFFFu;
-            if (sz == 0) break;                                                 // EndMark
-            if (sz > bs) { e.err = -4; break; }
-            const uint64_t at = ip;
-            if (n - ip < sz) { e.err = -1; break; }
-            ip += sz;
-            uint32_t sum = 0;
-            if (f.flg & 0x10) { if (n - ip < 4) { e.err = -1; break; } sum = rd32(src + ip); ip += 4; }
-            sink.block(at, word, sum);
-            f.nblocks++;
-        }
-        f.complete = !e.err;
-        f.has_checksum = !e.err && (f.flg & 4);
-        if (f.has_checksum) {
-            if (n - ip < 4) { e.err = -1; f.complete = false; f.has_checksum = false; }
-            else { f.content_checksum = rd32(src + ip); ip += 4; }
-        }
-        if (!f.complete) f.has_size = false;
-        sink.frame_end(f); e.seen = true;
-        if (single) { e.single_done = true; break; }                           // readSingleFrame (:83-91, 327, 346): the rest is not read
-        if (e.err) break;
-    }
-    e.ip = ip;
-    return e;
+    WalkPos pos{};
+    return walk_frames_from(src, n, ip, stop_at, single, pos, false, ~0ull, sink);
 }
 
 // The slot layout of the frame readers' decode (frame.cu's IndexSink, frame_streams.cu): a stored block needs its own size, a
@@ -216,6 +283,36 @@ struct FrameStreamRead {
 cudaError_t launch_frame_streams_walk(const FrameStreamRead& r, bool record, cudaStream_t st);
 // one warp per stream: result, consumed, content, and each block's k_dst / k_len (0 for a stream that fails)
 cudaError_t launch_frame_streams_verdict(const FrameStreamRead& r, cudaStream_t st);
+
+// The incremental reader (b200lz4f_reader_*: frame_reader_read_dev in frame.cu, kernels in frame_reader.cu).  A stream's
+// state between calls, host data that goes up with a call's arguments and comes back with its results: where its walk is,
+// the open frame's declared and counted content and its content checksum, and the latched status.
+static constexpr int32_t READER_MORE_INPUT = 0, READER_MORE_ROOM = 1, READER_DONE = 2;
+struct FrameReaderState {
+    uint64_t skip, declared, counted;                   // WalkPos.skip; the open frame's content size (FLG bit 3), content so far
+    Xxh32Carry xxh;                                     // the open frame's content checksum (FLG bit 2)
+    int32_t status;                                     // 0 while reading; READER_DONE or -1 .. -10 once latched
+    uint8_t where, flg, bd, seen;                       // WalkPos
+};
+// One call, all device pointers.  r holds the per-stream arguments and decode_dev's descriptor arrays as for
+// b200lz4f_decompress_streams_dev (r.consumed is src_consumed; r.result, r.content are unused).  Per block its unit's start in
+// the piece (k_at); per frame the part of it in this call (fr_mode READER_FR_*, where its header unit and its EndMark unit
+// start); per content-checksummed frame the carried checksum (f_carry, f_mode XXH_CARRY_*).
+enum { READER_FR_HEAD = 1, READER_FR_END = 2 };
+struct FrameReaderRead {
+    FrameStreamRead r;
+    const uint8_t* eof;
+    const FrameReaderState* st_in; FrameReaderState* st_out;
+    int32_t* status; uint64_t *produced, *need;
+    uint64_t* k_at;
+    uint64_t *fr_at, *fr_end_at; uint32_t* fr_mode;
+    Xxh32Carry* f_carry; uint8_t* f_mode;
+};
+// one thread per stream: with `record` false the counts (FS_* rows of r.cnt), the walk's end in tail / consumed / need /
+// st_out; with it every record
+cudaError_t launch_frame_reader_walk(const FrameReaderRead& q, bool record, cudaStream_t st);
+// one warp per stream: status, consumed, produced, need, st_out, and each block's k_dst / k_len (0 from the first failing unit)
+cudaError_t launch_frame_reader_verdict(const FrameReaderRead& q, cudaStream_t st);
 
 // ---- "LZ4Block" streams (LZ4BlockOutputStream.java:203-266, LZ4BlockInputStream.java:191-264).  The writer is the frame
 // writer's loop (compress_blocks_dev in containers.cu) with lz4block.cu's item sizes, emit and seal: the same FramePlan, a

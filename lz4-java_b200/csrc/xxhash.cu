@@ -358,16 +358,24 @@ __device__ __forceinline__ uint8_t ld_byte_l2(const uint8_t* p)
 __global__ void __launch_bounds__(32)
 xxh32_frames_chained_kernel(const uint8_t* __restrict__ slots, const uint64_t* __restrict__ blk_off, const uint32_t* __restrict__ f_first,
                             const uint32_t* __restrict__ f_nblk, const int32_t* __restrict__ blk_comp, const int32_t* __restrict__ blk_rawlen,
-                            const int32_t* c_res, uint32_t* __restrict__ out, uint32_t n)
+                            const int32_t* c_res, uint32_t* __restrict__ out, uint32_t n, Xxh32Carry* c_state = nullptr,
+                            const uint8_t* c_mode = nullptr)
 {
     __shared__ __align__(16) uint8_t s_carry[16];
     const uint32_t f = blockIdx.x;
     if (f >= n) return;
     const int lane = lane_id();
     const uint32_t first = f_first[f], nblk = f_nblk[f];
+    const uint32_t mode = c_mode ? c_mode[f] : 0u;          // XXH_CARRY_*: a frame that began or goes on in another call
     uint32_t v = xxh32_chain_init(0u, lane);
     uint64_t total = 0; uint32_t carry = 0;                 // bytes of the content seen so far; bytes waiting in s_carry
     bool big = false;                                       // at least one full stripe went through the chains
+    if (mode & XXH_CARRY_IN) {
+        const Xxh32Carry& c = c_state[f];
+        v = c.v[lane & 3]; total = c.total; carry = c.memsize; big = total >= 16;
+        if (uint32_t(lane) < carry) s_carry[lane] = c.mem[lane];
+        __syncwarp();
+    }
     for (uint32_t k = 0; k < nblk; k++) {
         const int32_t ci = blk_comp[first + k];
         int32_t r;
@@ -398,6 +406,13 @@ xxh32_frames_chained_kernel(const uint8_t* __restrict__ slots, const uint64_t* _
         if (uint32_t(lane) < carry) s_carry[lane] = ld_byte_l2(p + 16 * stripes + lane);
         __syncwarp();
     }
+    if (mode & XXH_CARRY_OUT) {                             // the frame goes on in a later call: its state, not its digest
+        Xxh32Carry& c = c_state[f];
+        if (lane < 4) c.v[lane] = v;
+        if (uint32_t(lane) < carry) c.mem[lane] = s_carry[lane];
+        if (lane == 0) { c.total = total; c.memsize = carry; }
+        return;
+    }
     const uint32_t h = big ? xxh32_chain_merge(v) : 0u + P32_5;
     if (lane == 0) out[f] = finish32(h + uint32_t(total), s_carry, carry);
 }
@@ -412,6 +427,18 @@ cudaError_t launch_xxh32_frames_chained(const uint8_t* slots, const uint64_t* bl
     return cudaGetLastError();
 }
 #endif
+// the incremental reader's launch (frame_reader.cu): the same code in the emulator build (B200_LAUNCH), where the decoder has
+// finished before this runs and nothing spins
+cudaError_t launch_xxh32_frames_chained_carry(const uint8_t* slots, const uint64_t* blk_off, const uint32_t* f_first,
+                                              const uint32_t* f_nblk, const int32_t* blk_comp, const int32_t* blk_rawlen,
+                                              const int32_t* c_res, uint32_t* out, size_t n, Xxh32Carry* carry,
+                                              const uint8_t* mode, cudaStream_t st)
+{
+    if (n == 0) return cudaSuccess;
+    B200_LAUNCH(xxh32_frames_chained_kernel, (unsigned)n, 32, st, slots, blk_off, f_first, f_nblk, blk_comp, blk_rawlen, c_res, out,
+                (uint32_t)n, carry, mode);
+    return cudaGetLastError();
+}
 
 // ---- the same for XXH64: stripes of 32 bytes, rows of 256 bytes (one 64-bit word per lane), chain = lane & 3.
 __device__ __forceinline__ uint64_t xxh64_chain_init(uint64_t seed, int lane)

@@ -163,6 +163,73 @@ def decompress_frame_streams_dev(src, src_off, src_len, out, dst_off, dst_cap, r
     return result, consumed, content
 
 
+MORE_INPUT, MORE_ROOM, DONE = 0, 1, 2
+
+
+class FrameReader:
+    """ns LZ4 frame streams read piece by piece in device memory, each one LZ4FrameInputStream(in, readSingleFrame) whose
+    bytes arrive over time (b200lz4f_reader_*).  The reader is host data, the streams' carried state; not thread-safe.
+
+        with FrameReader(ns) as rd:
+            status, consumed, produced, need = rd.read(src, src_off, src_len, out, dst_off, dst_cap, eof)
+
+    A call takes the complete units at the start of stream s's piece src[src_off[s] : src_off[s] + src_len[s]] and packs their
+    content into out[dst_off[s] : dst_off[s] + produced[s]], never past dst_cap[s].  The next piece of stream s must start
+    at byte consumed[s] of this one.  status[s]: MORE_INPUT (need[s]: bytes the next unit takes), MORE_ROOM (need[s]: the room
+    the next block takes), DONE, or the LZ4FrameError code -1 .. -10, after the content in front of the failing unit was
+    delivered.  eof[s] true: the piece ends the stream.  DONE and errors are latched.  src, out: contiguous uint8 CUDA tensors
+    on one device; the rest: host sequences.  Runs on torch's current stream and returns when the results are on the host.
+    -> (status, consumed, produced, need): np.int32 / np.uint64 arrays."""
+
+    def __init__(self, ns: int, read_single_frame: bool = False):
+        import ctypes
+        err = ctypes.c_int(0)
+        self.ns = int(ns)
+        self._h = N.lib().b200lz4f_reader_create(self.ns, int(bool(read_single_frame)), ctypes.byref(err))
+        if not self._h:
+            N.check(err.value)
+            raise MemoryError("b200lz4f_reader_create")
+
+    def read(self, src, src_off, src_len, out, dst_off, dst_cap, eof):
+        import torch
+        if not self._h:
+            raise ValueError("the reader is closed")
+        off, ln = _dev_streams(src, src_off, src_len, "piece")
+        if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+            raise ValueError("out must be a contiguous uint8 tensor on src's device")
+        doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+        dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+        end = np.ascontiguousarray(np.asarray(eof, dtype=bool).reshape(-1)).astype(np.uint8)
+        if len(ln) != self.ns or len(doff) != self.ns or len(dcap) != self.ns or len(end) != self.ns:
+            raise ValueError(f"src_off, src_len, dst_off, dst_cap and eof must have one entry per stream ({self.ns})")
+        if self.ns and int((doff + dcap).max()) > out.numel():
+            raise ValueError("a destination range reaches past the end of out")
+        status = np.zeros(self.ns, dtype=np.int32)
+        consumed, produced, need = (np.zeros(self.ns, dtype=np.uint64) for _ in range(3))
+        N.check(N.lib().b200lz4f_reader_read_dev(self._h, src.data_ptr(), off.ctypes.data, ln.ctypes.data, end.ctypes.data,
+                                                 out.data_ptr(), doff.ctypes.data, dcap.ctypes.data, status.ctypes.data,
+                                                 consumed.ctypes.data, produced.ctypes.data, need.ctypes.data,
+                                                 torch.cuda.current_stream(src.device).cuda_stream))
+        return status, consumed, produced, need
+
+    def close(self):
+        if self._h:
+            N.lib().b200lz4f_reader_free(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ---- lz4-java's private "LZ4Block" container (LZ4BlockOutputStream / LZ4BlockInputStream)
 def compress_lz4block(src, block_size: int = 1 << 16, hc_level: int = 0) -> bytes:
     s = _view(src)
