@@ -329,6 +329,44 @@ void    b200lz4f_reader_free(void* reader);
 int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t nf,
                               uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
                               int bsCode, int flags, int hc_level, void* stream);
+/* Incremental device-resident LZ4 Frame writer for ns streams, each one LZ4FrameOutputStream(out, BLOCKSIZE(bsCode),
+ * knownSize, compressor, bits) whose content arrives in pieces (LZ4FrameOutputStream.java:178-306): the incremental
+ * counterpart of b200lz4f_compress_dev, built from the same parts.  bsCode / flags / hc_level as b200lz4f_compress_dev takes
+ * them, for every stream.  A writer (b200lz4f_writer_create) is host data, a few dozen bytes of state per stream; create and
+ * free make no CUDA call.  It returns NULL with *err = B200LZ4_E_ARG for a bsCode outside 4..7, ns above 2^31 - 1, or, with
+ * flags bit 2, a NULL known_size (HOST array of ns declared content sizes) or an entry below 0 (the constructor's
+ * IllegalArgumentException).  Any thread may use a writer, one at a time (it is not thread-safe, like LZ4FrameOutputStream).
+ * b200lz4f_writer_write_dev: stream s's next piece is src_len[s] bytes at d_src + src_off[s]; its frame bytes go to d_dst +
+ * dst_off[s] with room dst_cap[s]; op[s] is B200LZ4F_WRITE, _FLUSH or _CLOSE (HOST arrays of ns entries; the bytes device
+ * memory of the current device).  Per stream:
+ *  - The stream's first call with room for it writes the header (content size known_size[s]).  Then the call takes whole
+ *    blocks of blockMaxSize from the start of the piece; with FLUSH or CLOSE the rest of the piece as one short block (none
+ *    when nothing is left, as flush() writes none); with CLOSE then the EndMark and the content checksum.
+ *  - A unit is taken only while the room left holds its bound: a block 4 + its length (+ 4 with block checksums), the header
+ *    7 or 15 bytes, the EndMark 4 or 8.  The bytes go to [dst_off[s], dst_off[s] + produced[s]), never past dst_cap[s].
+ *  - src_consumed[s] is the bytes taken.  The rest of the piece is the caller's to present again at the start of the next
+ *    one: the writer keeps no payload byte between calls.
+ *  - status[s]: B200LZ4F_MORE_INPUT (everything takeable was taken; need[s] = the bytes missing for the next whole block,
+ *    blockMaxSize after a flush), B200LZ4F_MORE_ROOM (need[s] = the bound of the unit that did not fit; a CLOSE that ran out
+ *    of room is repeated), B200LZ4F_DONE (closed; latched: later calls take and produce nothing).  known_size is not checked
+ *    against the content, as LZ4FrameOutputStream does not check it: a mismatch gives a frame the readers answer with -8.
+ *  - The concatenated output of stream s is byte for byte what LZ4FrameOutputStream writes for the same content with
+ *    flush() where FLUSH was passed, each block compressed by the library's block compressor at the 16-byte phase where the
+ *    call found it; with no FLUSH and pieces at the phase of the whole content, the frame b200lz4f_compress_dev writes for it.
+ *    The content checksum travels in the state, so frames of any length are checksummed.
+ * Returns 0 or B200LZ4_E_*: a NULL writer or pointer, an op above _CLOSE, a destination range that overflows or more than
+ * 2^31 - 1 blocks in one call are found before anything is launched or written.  The launches depend on the number of
+ * chunks, not on ns or the number of blocks; one synchronisation; only the plan, the ranges written and the checksum states
+ * cross PCIe.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep
+ * scratch of the thread's context (the frame writer's), sized by the call, never by how much a stream has written. */
+#define B200LZ4F_WRITE 0      /* take whole blocks only                                  */
+#define B200LZ4F_FLUSH 1      /* ... and the rest of the piece as a short block (flush()) */
+#define B200LZ4F_CLOSE 2      /* ... then the EndMark and content checksum (close())      */
+void*   b200lz4f_writer_create(size_t ns, int bsCode, int flags, int hc_level, const int64_t* known_size, int* err);
+int     b200lz4f_writer_write_dev(void* writer, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                  const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                  int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream);
+void    b200lz4f_writer_free(void* writer);
 
 /* ---------------------------------------------------------------- lz4-java's containers as whole-buffer calls
  * LZ4 Frame writer (LZ4FrameOutputStream.java:178-251): independent blocks of 64 KiB..4 MiB (bsCode 4..7), blocks that

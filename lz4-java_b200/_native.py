@@ -80,6 +80,9 @@ SYMBOLS = [
     ("b200lz4f_reader_read_dev", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     ("b200lz4f_reader_free", None, [_vp]),
     ("b200lz4f_compress_dev", C.c_int64, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _i, _i, _i, _vp]),
+    ("b200lz4f_writer_create", _vp, [_sz, _i, _i, _i, _vp, _vp]),
+    ("b200lz4f_writer_write_dev", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    ("b200lz4f_writer_free", None, [_vp]),
     ("b200lz4f_compress_bound", _sz, [_sz, _i]),
     ("b200lz4f_compress_host", C.c_int64, [_vp, _sz, _vp, _sz, _i, _i]),
     ("b200lz4f_compress_host_hc", C.c_int64, [_vp, _sz, _vp, _sz, _i, _i, _i]),

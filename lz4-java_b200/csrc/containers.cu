@@ -14,6 +14,7 @@
 #include "kernels.h"
 #ifdef B200_HOST_SIM            // the emulator build compiles the host layer only: the device writers' and readers' kernels come with it
 #include "frame_encode.cu"
+#include "frame_writer.cu"
 #include "lz4block.cu"
 #include "with_length.cu"
 #endif
@@ -29,18 +30,22 @@ namespace b200 {
 
 // Where the FramePlan arrays of a call with nb blocks, ni items and nf frames lie in one blob, the same on the host and the
 // device.  f_off, f_end and the two carry words come last: one copy brings the results back.
+// The incremental writer (nw = nf) adds per frame where its stream's range starts, its first item, its WRITER_* mode and its
+// declared content size, and (nx = nf with a content checksum) the carried checksum's mode and state, which comes back too;
+// the other writers have none of these (nw = nx = 0), and their layout is the same without them.
 struct FramePlanLayout {
     size_t b_soff, b_slen, b_slot, b_ccap, b_clen, b_poff, b_plen, b_sum;
     size_t i_frame, i_block, i_size, i_off;
-    size_t f_soff, f_len, f_len32, f_sum, f_off, f_end, carry, bytes = 0;
-    FramePlanLayout(size_t nb, size_t ni, size_t nf)
+    size_t f_soff, f_len, f_len32, f_sum, f_doff, f_first, f_mode, f_known, f_xmode, f_off, f_end, f_xxh, carry, bytes = 0;
+    FramePlanLayout(size_t nb, size_t ni, size_t nf, size_t nw = 0, size_t nx = 0)
     {
         auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
         b_soff = take(8 * nb); b_slen = take(4 * nb); b_slot = take(8 * nb); b_ccap = take(4 * nb); b_clen = take(4 * nb);
         b_poff = take(8 * nb); b_plen = take(4 * nb); b_sum = take(4 * nb);
         i_frame = take(4 * ni); i_block = take(4 * ni); i_size = take(4 * ni); i_off = take(8 * ni);
         f_soff = take(8 * nf); f_len = take(8 * nf); f_len32 = take(4 * nf); f_sum = take(4 * nf);
-        f_off = take(8 * nf); f_end = take(8 * nf); carry = take(16);
+        f_doff = take(8 * nw); f_first = take(4 * nw); f_mode = take(nw); f_known = take(8 * nw); f_xmode = take(nx);
+        f_off = take(8 * nf); f_end = take(8 * nf); f_xxh = take(sizeof(Xxh32Carry) * nx); carry = take(16);
     }
 };
 
@@ -54,43 +59,16 @@ enum class Container { Frame, LZ4Block, WithLength };
 
 static constexpr uint64_t LZ4_MAX_INPUT = 0x7E000000;              // LZ4_MAX_INPUT_SIZE (lz4.h:211)
 
-// Every writer: arguments and sizes (nothing is launched or written before these pass), the plan, the chunk loop and the
-// results.  Only the item sizes, the emit, the checksums and the seal differ by container.  bs: bytes per block (WithLength:
-// more than any record); code: the frame's bsCode or the LZ4Block token's level nibble; flags: the frame's (0 otherwise).
-static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
-                                   size_t nf, uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
-                                   uint64_t bs, int code, int flags, int hc_level, cudaStream_t st)
+// The plan of a writer call, into the pinned blob H laid out by L: frame f is src_len[f] bytes at src_off[f], cut into blocks
+// of bs bytes (the last one short; a record is one block), one item per block or one item for an empty frame, and chunks of
+// at most CHUNK_SPAN source bytes and CHUNK_BLOCKS items, so the compressed slots take the same room however large the call.
+// Returns the slot room the largest chunk takes.
+static uint64_t plan_blocks(Container kind, const FramePlanLayout& L, uint8_t* H, const uint64_t* src_off, const uint64_t* src_len,
+                            size_t nf, uint64_t bs, std::vector<FrameChunk>& chunks)
 {
-    const bool frame = kind == Container::Frame, rec = kind == Container::WithLength;
-    if (nf == 0) return 0;
-    if (!src_off || !src_len || !d_dst) return fail_arg("null pointer");
-    uint64_t need = 0, nb = 0, ni = 0, bytes = 0;
-    bool too_long = false;
-    for (size_t f = 0; f < nf; f++) {
-        const uint64_t n = src_len[f];
-        if (n > (1ull << 47)) return fail_arg("src_len");
-        if (rec && n > LZ4_MAX_INPUT) return fail_arg("a record is at most 0x7E000000 bytes");
-        const uint64_t nbf = rec ? 1 : (n + bs - 1) / bs;
-        need += frame ? b200lz4f_compress_bound(n, code) : rec ? 4 + compress_bound(n) : b200lz4block_compress_bound(n, (int)bs);
-        nb += nbf; ni += nbf ? nbf : 1; bytes += n;
-        if ((flags & 1) && n > 0x7FFFFFFFull) too_long = true;
-    }
-    if (bytes && !d_src) return fail_arg("null pointer");
-    if (ni > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
-    if (need > dst_capacity) return -9;
-    if (too_long) return -10;                                       // the content checksum kernel takes 31-bit lengths (f_len32)
-    FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
-    const FramePlanLayout L(nb, ni, nf);
-    rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
-    if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
-    if (rc) return rc;
-
-    // ---- plan: blocks of bs bytes (the last one of a frame short), items, and chunks of at most CHUNK_SPAN source bytes and
-    // CHUNK_BLOCKS items, so the compressed slots take the same room however large the call
-    uint8_t* H = s->h_plan;
+    const bool rec = kind == Container::WithLength;
     auto h64 = [&](size_t o) { return (uint64_t*)(H + o); };
     auto h32 = [&](size_t o) { return (int32_t*)(H + o); };
-    std::vector<FrameChunk> chunks;
     size_t b = 0, i = 0, ci0 = 0, cb0 = 0;
     uint64_t slot = 0, span = 0, slots_need = 0;
     // A chunk's blocks go to the wide compressor when they are at most 64 KiB (as b200lz4_compress_default picks it), else to
@@ -136,8 +114,70 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
         }
     }
     close_chunk(i);
-    slots_need = slot > slots_need ? slot : slots_need;
     h64(L.carry)[0] = 0;
+    return slot > slots_need ? slot : slots_need;
+}
+
+// The chunk loop of every writer, ordered on st: per chunk the blocks are compressed into their slots, then the container's
+// item sizes (sizes(i0, n)), the scan that places the items (the running offset carried from chunk to chunk in carry[0..1])
+// and the container's emit (emit(i0, n)).  b_ccap: the blocks' slot capacities.
+template <class Sizes, class Emit>
+static int chunk_loop(const FramePlan& P, const int32_t* b_ccap, uint8_t* slots, const std::vector<FrameChunk>& chunks, int hc_level,
+                      uint64_t* carry, Sizes sizes, Emit emit, cudaStream_t st)
+{
+    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+    auto blocks = [&](size_t b0, size_t b1) {
+        return BatchArgs{ P.src, P.b_soff + b0, P.b_slen + b0, slots, P.b_slot + b0, b_ccap + b0, (int32_t*)P.b_clen + b0, b1 - b0 };
+    };
+    for (size_t k = 0; k < chunks.size(); k++) {
+        const FrameChunk& c = chunks[k];
+        // the stream's compressor argument: hc_level 0 = the fast compressor, 1..17 = HC
+        if (hc_level > 0 && c.b1 > c.b0) CK(counted(launch_compress_hc(blocks(c.b0, c.b1), hc_level, st)));
+        if (hc_level <= 0 && c.bw > c.b0) CK(counted(launch_compress_fast(blocks(c.b0, c.bw), 65536, st)));
+        if (hc_level <= 0 && c.b1 > c.bw) CK(counted(launch_compress_fast(blocks(c.bw, c.b1), 0, st)));
+        const uint32_t i0 = (uint32_t)c.i0, n = (uint32_t)(c.i1 - c.i0);
+        CK(counted(sizes(i0, n)));
+        CK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
+        CK(counted(emit(i0, n)));
+    }
+    return 0;
+}
+
+// Every writer: arguments and sizes (nothing is launched or written before these pass), the plan, the chunk loop and the
+// results.  Only the item sizes, the emit, the checksums and the seal differ by container.  bs: bytes per block (WithLength:
+// more than any record); code: the frame's bsCode or the LZ4Block token's level nibble; flags: the frame's (0 otherwise).
+static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                   size_t nf, uint8_t* d_dst, size_t dst_capacity, uint64_t* frame_off, uint64_t* frame_len,
+                                   uint64_t bs, int code, int flags, int hc_level, cudaStream_t st)
+{
+    const bool frame = kind == Container::Frame, rec = kind == Container::WithLength;
+    if (nf == 0) return 0;
+    if (!src_off || !src_len || !d_dst) return fail_arg("null pointer");
+    uint64_t need = 0, nb = 0, ni = 0, bytes = 0;
+    bool too_long = false;
+    for (size_t f = 0; f < nf; f++) {
+        const uint64_t n = src_len[f];
+        if (n > (1ull << 47)) return fail_arg("src_len");
+        if (rec && n > LZ4_MAX_INPUT) return fail_arg("a record is at most 0x7E000000 bytes");
+        const uint64_t nbf = rec ? 1 : (n + bs - 1) / bs;
+        need += frame ? b200lz4f_compress_bound(n, code) : rec ? 4 + compress_bound(n) : b200lz4block_compress_bound(n, (int)bs);
+        nb += nbf; ni += nbf ? nbf : 1; bytes += n;
+        if ((flags & 1) && n > 0x7FFFFFFFull) too_long = true;
+    }
+    if (bytes && !d_src) return fail_arg("null pointer");
+    if (ni > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
+    if (need > dst_capacity) return -9;
+    if (too_long) return -10;                                       // the content checksum kernel takes 31-bit lengths (f_len32)
+    FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
+    const FramePlanLayout L(nb, ni, nf);
+    rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
+    if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
+    if (rc) return rc;
+
+    uint8_t* H = s->h_plan;
+    auto h64 = [&](size_t o) { return (uint64_t*)(H + o); };
+    std::vector<FrameChunk> chunks;
+    const uint64_t slots_need = plan_blocks(kind, L, H, src_off, src_len, nf, bs, chunks);
     rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
 
     uint8_t* D = s->d_plan;
@@ -167,23 +207,12 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
                 d_src, P.b_soff, P.b_slen, LZ4BLOCK_SEED, (uint32_t*)P.b_sum, (size_t)nb, side->st)));
         CK(cudaEventRecord(side->join, side->st));
     }
-    auto blocks = [&](size_t b0, size_t b1) {
-        return BatchArgs{ d_src, P.b_soff + b0, P.b_slen + b0, s->d_slots, P.b_slot + b0,
-                          (const int32_t*)(D + L.b_ccap) + b0, (int32_t*)P.b_clen + b0, b1 - b0 };
-    };
-    for (size_t k = 0; k < chunks.size(); k++) {
-        const FrameChunk& c = chunks[k];
-        // the stream's compressor argument: hc_level 0 = the fast compressor, 1..17 = HC
-        if (hc_level > 0 && c.b1 > c.b0) CK(counted(launch_compress_hc(blocks(c.b0, c.b1), hc_level, st)));
-        if (hc_level <= 0 && c.bw > c.b0) CK(counted(launch_compress_fast(blocks(c.b0, c.bw), 65536, st)));
-        if (hc_level <= 0 && c.b1 > c.bw) CK(counted(launch_compress_fast(blocks(c.bw, c.b1), 0, st)));
-        const uint32_t i0 = (uint32_t)c.i0, n = (uint32_t)(c.i1 - c.i0);
-        CK(counted(frame ? launch_frame_sizes(P, i0, n, st) : rec ? launch_with_length_sizes(P, i0, n, st)
-                                                                  : launch_lz4block_sizes(P, i0, n, st)));
-        CK(counted(launch_scan(P.i_size + i0, P.i_off + i0, carry + ((k + 1) & 1), carry + (k & 1), n, st)));
-        CK(counted(frame ? launch_frame_emit(P, i0, n, st) : rec ? launch_with_length_emit(P, i0, n, st)
-                                                                 : launch_lz4block_emit(P, i0, n, st)));
-    }
+    rc = chunk_loop(P, (const int32_t*)(D + L.b_ccap), s->d_slots, chunks, hc_level, carry,
+                    [&](uint32_t i0, uint32_t n) { return frame ? launch_frame_sizes(P, i0, n, st) : rec ? launch_with_length_sizes(P, i0, n, st)
+                                                                                                         : launch_lz4block_sizes(P, i0, n, st); },
+                    [&](uint32_t i0, uint32_t n) { return frame ? launch_frame_emit(P, i0, n, st) : rec ? launch_with_length_emit(P, i0, n, st)
+                                                                                                        : launch_lz4block_emit(P, i0, n, st); }, st);
+    if (rc) return rc;
     if ((flags & 2) && nb) {        // block checksums over the payloads as written; the source average bounds the payloads'
         CK(counted((bytes / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
             d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
@@ -230,6 +259,145 @@ static int64_t compress_with_length_dev(const uint8_t* d_src, const uint64_t* sr
 {   // one block per record: bs is longer than any record may be
     return compress_blocks_dev(Container::WithLength, d_src, src_off, src_len, n, d_dst, dst_capacity, rec_off, rec_len,
                                1ull << 31, 0, 0, hc_level, st);
+}
+
+// ---- the incremental frame writer (b200lz4f_writer_*; kernels: frame_writer.cu).  The writer is host data: the streams'
+// declared content sizes and one state each.
+struct FrameWriterHandle {
+    size_t ns; int bsCode, flags, hc_level;
+    std::vector<uint64_t> known;
+    std::vector<FrameWriterState> st;
+};
+
+// What a call does for one stream, planned on the host from its piece's length, its op, its room and its state alone: the
+// header if it is due and fits, then whole blocks while their bounds fit, the short tail at FLUSH / CLOSE, the EndMark at
+// CLOSE.  mode: WRITER_* for the plan.
+struct WriterTake { uint64_t taken, need; int32_t status; uint8_t mode; };
+static WriterTake writer_take(const FrameWriterState& w, uint64_t n, uint8_t op, uint64_t room, uint64_t bs, int flags)
+{
+    if (w.done) return { 0, 0, B200LZ4F_DONE, 0 };
+    const uint64_t head = 7 + ((flags & 4) ? 8 : 0), tail = 4 + ((flags & 1) ? 4 : 0), word = 4 + ((flags & 2) ? 4 : 0);
+    WriterTake t{ 0, 0, B200LZ4F_MORE_ROOM, 0 };
+    if (!w.head) {                                                      // writeHeader (:178-191)
+        if (room < head) { t.need = head; return t; }
+        room -= head; t.mode |= WRITER_HEAD;
+    }
+    const uint64_t whole = n / bs, fit = room / (bs + word), k = whole < fit ? whole : fit;
+    t.taken = k * bs; room -= k * (bs + word);
+    if (k < whole) { t.need = bs + word; return t; }
+    const uint64_t rest = n - t.taken;
+    if (op != B200LZ4F_WRITE && rest) {                                 // flush(): the rest as a short block (:199-241)
+        if (room < rest + word) { t.need = rest + word; return t; }
+        t.taken = n; room -= rest + word;
+    }
+    if (op == B200LZ4F_CLOSE) {                                         // close(): writeEndMark (:243-249)
+        if (room < tail) { t.need = tail; return t; }
+        t.mode |= WRITER_TAIL; t.status = B200LZ4F_DONE; return t;
+    }
+    t.status = B200LZ4F_MORE_INPUT; t.need = op == B200LZ4F_WRITE ? bs - rest : bs;
+    return t;
+}
+
+// compress_blocks_dev's plan and chunk loop over the streams that write something, with frame_writer.cu's item kernels: the
+// plan up, the carried content checksums on the side stream from the start, the chunks, the block checksums, the seal, each
+// stream's range and checksum state back, one synchronisation.
+static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                  const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                  int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
+{
+    if (!h) return fail_arg("null writer");
+    const size_t ns = h->ns;
+    if (ns == 0) return 0;
+    if (!src_off || !src_len || !op || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
+        return fail_arg("null pointer");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+        if (op[k] > B200LZ4F_CLOSE) return fail_arg("op must be B200LZ4F_WRITE, _FLUSH or _CLOSE");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    const int flags = h->flags;
+    const uint64_t bs = 1ull << (8 + 2 * h->bsCode);
+    std::vector<WriterTake> take(ns);
+    std::vector<uint64_t> p_soff, p_len;
+    std::vector<uint32_t> p_stream;
+    uint64_t nb = 0, ni = 0, taken = 0;
+    for (size_t k = 0; k < ns; k++) {
+        take[k] = writer_take(h->st[k], src_len[k], op[k], dst_cap[k], bs, flags);
+        if (!take[k].mode && !take[k].taken) continue;
+        const uint64_t nbf = (take[k].taken + bs - 1) / bs;
+        p_soff.push_back(src_off[k]); p_len.push_back(take[k].taken); p_stream.push_back((uint32_t)k);
+        nb += nbf; ni += nbf ? nbf : 1; taken += take[k].taken;
+    }
+    if (ni > 0x7FFFFFFFull) return fail_arg("more than 2^31 - 1 blocks in one call");
+    const size_t nf = p_stream.size(), nx = (flags & 1) ? nf : 0;
+    std::vector<uint64_t> range(ns, 0);
+    std::vector<Xxh32Carry> xxh;
+    if (nf) {
+        FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
+        const FramePlanLayout L(nb, ni, nf, nf, nx);
+        rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
+        if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
+        if (rc) return rc;
+        uint8_t *H = s->h_plan, *D = s->d_plan;
+        std::vector<FrameChunk> chunks;
+        const uint64_t slots_need = plan_blocks(Container::Frame, L, H, p_soff.data(), p_len.data(), nf, bs, chunks);
+        rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
+        for (size_t f = 0, i = 0; f < nf; f++) {
+            const size_t k = p_stream[f];
+            ((uint64_t*)(H + L.f_doff))[f] = dst_off[k];
+            ((uint32_t*)(H + L.f_first))[f] = (uint32_t)i;
+            (H + L.f_mode)[f] = take[k].mode;
+            ((uint64_t*)(H + L.f_known))[f] = h->known.empty() ? 0 : h->known[k];
+            if (nx) {                                                   // the checksum goes on, or ends in its digest
+                (H + L.f_xmode)[f] = XXH_CARRY_IN | ((take[k].mode & WRITER_TAIL) ? 0 : XXH_CARRY_OUT);
+                ((Xxh32Carry*)(H + L.f_xxh))[f] = h->st[k].xxh;
+            }
+            i += p_len[f] ? (p_len[f] + bs - 1) / bs : 1;
+        }
+        const FramePlan P{ d_src, d_dst, s->d_slots,
+                           (const uint64_t*)(D + L.b_soff), (const int32_t*)(D + L.b_slen), (const uint64_t*)(D + L.b_slot), (const int32_t*)(D + L.b_clen),
+                           (uint64_t*)(D + L.b_poff), (int32_t*)(D + L.b_plen), (const uint32_t*)(D + L.b_sum),
+                           (const uint32_t*)(D + L.i_frame), (const int32_t*)(D + L.i_block), (int32_t*)(D + L.i_size), (uint64_t*)(D + L.i_off),
+                           (const uint64_t*)(D + L.f_known), (const uint32_t*)(D + L.f_sum), (uint64_t*)(D + L.f_off), (uint64_t*)(D + L.f_end),
+                           (uint32_t)ni, h->bsCode, flags, 0 };
+        const FrameWriterPlan W{ P, (const uint64_t*)(D + L.f_doff), (const uint32_t*)(D + L.f_first), (const uint8_t*)(D + L.f_mode) };
+
+        Drain drain{ st, side->st };
+        auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+        CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
+        if (nx) {                   // the content checksums of the runs taken, from the start, beside everything else
+            CK(cudaEventRecord(side->fork, st));
+            CK(cudaStreamWaitEvent(side->st, side->fork, 0));
+            CK(counted(launch_xxh32_long_carry(d_src, (const uint64_t*)(D + L.f_soff), (const uint64_t*)(D + L.f_len),
+                                               (uint32_t*)(D + L.f_sum), (Xxh32Carry*)(D + L.f_xxh), D + L.f_xmode, nf, side->st)));
+            CK(cudaEventRecord(side->join, side->st));
+        }
+        rc = chunk_loop(P, (const int32_t*)(D + L.b_ccap), s->d_slots, chunks, h->hc_level, (uint64_t*)(D + L.carry),
+                        [&](uint32_t i0, uint32_t n) { return launch_frame_writer_sizes(W, i0, n, st); },
+                        [&](uint32_t i0, uint32_t n) { return launch_frame_writer_emit(W, i0, n, st); }, st);
+        if (rc) return rc;
+        if ((flags & 2) && nb) {    // block checksums over the payloads as written, as compress_blocks_dev takes them
+            CK(counted((taken / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+                d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
+        }
+        if (nx) CK(cudaStreamWaitEvent(st, side->join, 0));
+        CK(counted(launch_frame_writer_seal(W, st)));
+        CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        drain.done = true;
+        for (size_t f = 0; f < nf; f++) range[p_stream[f]] = ((const uint64_t*)(H + L.f_end))[f] - ((const uint64_t*)(H + L.f_off))[f];
+        if (nx) xxh.assign((const Xxh32Carry*)(H + L.f_xxh), (const Xxh32Carry*)(H + L.f_xxh) + nf);
+    }
+    for (size_t k = 0; k < ns; k++) {
+        status[k] = take[k].status; src_consumed[k] = take[k].taken; produced[k] = range[k]; need[k] = take[k].need;
+        if (take[k].mode & WRITER_HEAD) h->st[k].head = 1;
+        if (take[k].status == B200LZ4F_DONE) h->st[k].done = 1;
+    }
+    for (size_t f = 0; f < xxh.size(); f++) h->st[p_stream[f]].xxh = xxh[f];
+    return 0;
 }
 
 // A device writer, write(d_src, src_off, src_len, d_dst, capacity, st) for one source, run on a copy of src in the thread's
@@ -470,6 +638,39 @@ int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, si
 }
 int64_t b200lz4f_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags)
 { return b200lz4f_compress_host_hc(src, n, dst, cap, bsCode, flags, 0); }
+
+// the incremental writer (frame_writer_write_dev): host data only, no CUDA call in create or free
+void* b200lz4f_writer_create(size_t ns, int bsCode, int flags, int hc_level, const int64_t* known_size, int* err)
+{
+    if (err) *err = 0;
+    auto fail = [&](const char* what) -> void* { const int rc = b200::fail_arg(what); if (err) *err = rc; return nullptr; };
+    if (bsCode < 4 || bsCode > 7) return fail("bsCode must be 4..7");
+    if (ns > 0x7FFFFFFFull) return fail("too many streams in one writer");
+    if (flags & 4) {                // LZ4FrameOutputStream's constructor: a declared size needs a known one (:138-140)
+        if (ns && !known_size) return fail("known_size is needed with flags bit 2");
+        for (size_t k = 0; k < ns; k++) if (known_size[k] < 0) return fail("known_size must be >= 0");
+    }
+    b200::FrameWriterHandle* h = new (std::nothrow) b200::FrameWriterHandle;
+    if (!h) return fail("out of host memory");
+    h->ns = ns; h->bsCode = bsCode; h->flags = flags; h->hc_level = hc_level;
+    try {
+        if (flags & 4) h->known.assign((const uint64_t*)known_size, (const uint64_t*)known_size + ns);
+        b200::FrameWriterState w{};                 // XXH32 with seed 0, nothing hashed yet (xxhash.c:445-455)
+        w.xxh.v[0] = 2654435761u + 2246822519u; w.xxh.v[1] = 2246822519u; w.xxh.v[2] = 0; w.xxh.v[3] = 0u - 2654435761u;
+        h->st.assign(ns, w);
+    } catch (...) { delete h; return fail("out of host memory"); }
+    return h;
+}
+
+int b200lz4f_writer_write_dev(void* writer, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                              const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                              int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream)
+{
+    return b200::frame_writer_write_dev((b200::FrameWriterHandle*)writer, d_src, src_off, src_len, op, d_dst, dst_off, dst_cap,
+                                        status, src_consumed, produced, need, (cudaStream_t)stream);
+}
+
+void b200lz4f_writer_free(void* writer) { delete (b200::FrameWriterHandle*)writer; }
 
 // ---------------------------------------------------------------- "LZ4Block" container
 size_t b200lz4block_compress_bound(size_t n, int blockSize)

@@ -49,6 +49,11 @@ cudaError_t launch_xxh32_frames_chained_carry(const uint8_t* slots, const uint64
                                               const uint8_t* mode, cudaStream_t st);
 cudaError_t launch_xxh64(const uint8_t* base, const uint64_t* off, const int32_t* len, uint64_t seed,
                          uint64_t* out, size_t n, cudaStream_t st);
+// launch_xxh32_long (seed 0) with 64-bit lengths and a carried state per run (the incremental writer, frame_writer.cu): run r
+// is len[r] bytes at base + off[r]; mode[r] XXH_CARRY_IN starts from carry[r] (else a fresh state), XXH_CARRY_OUT leaves the
+// state in carry[r] (else the digest goes to out[r]).  One warp per run; one launcher for both builds (B200_LAUNCH).
+cudaError_t launch_xxh32_long_carry(const uint8_t* base, const uint64_t* off, const uint64_t* len, uint32_t* out, Xxh32Carry* carry,
+                                    const uint8_t* mode, size_t n, cudaStream_t st);
 
 // streaming hash: one device-resident state per handle, updated by a single-warp kernel
 struct Xxh32State { uint64_t total; uint32_t v[4]; uint8_t mem[16]; uint32_t memsize; uint32_t seed; uint32_t digest; };
@@ -94,6 +99,25 @@ cudaError_t launch_frame_sizes(const FramePlan& p, uint32_t i0, uint32_t n, cuda
 cudaError_t launch_frame_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
 // every item: headers, block checksums, EndMarks, content checksums, f_off / f_end (frame_seal_kernel)
 cudaError_t launch_frame_seal(const FramePlan& p, cudaStream_t st);
+
+// The incremental frame writer (b200lz4f_writer_*: frame_writer_write_dev in containers.cu, kernels in frame_writer.cu).  One
+// call is the frame writer's plan and chunk loop over the streams that write something: a "frame" of the plan is one such
+// stream's part of the call (its blocks, or one item without a block), with the header only on the stream's first call
+// (WRITER_HEAD) and the EndMark and content checksum only at its close (WRITER_TAIL).  Each stream's bytes go to its own
+// range: item i of plan frame f lands at f_doff[f] + i_off[i] - i_off[f_first[f]].  p.f_len is the declared content size;
+// f_off / f_end come back as the stream's range written.
+enum { WRITER_HEAD = 1, WRITER_TAIL = 2 };
+struct FrameWriterPlan {
+    FramePlan p;
+    const uint64_t* f_doff; const uint32_t* f_first; const uint8_t* f_mode;
+};
+// items [i0, i0 + n): their sizes, and their block words and payloads (one warp each)
+cudaError_t launch_frame_writer_sizes(const FrameWriterPlan& w, uint32_t i0, uint32_t n, cudaStream_t st);
+cudaError_t launch_frame_writer_emit(const FrameWriterPlan& w, uint32_t i0, uint32_t n, cudaStream_t st);
+// every item: headers, block checksums, EndMarks, content checksums, f_off / f_end
+cudaError_t launch_frame_writer_seal(const FrameWriterPlan& w, cudaStream_t st);
+// A stream's state between calls, host data: its carried content checksum, whether its header is out, whether it is closed.
+struct FrameWriterState { Xxh32Carry xxh; uint8_t head, done, pad[6]; };
 
 // ---- LZ4 Frame reader: the container walk (LZ4FrameInputStream.nextFrameInfo / readHeader / readBlock as an index pass,
 // LZ4FrameInputStream.java:132-321).  The host indexer (frame.cu) and the device one (frame_index.cu) both run walk_frames;

@@ -334,6 +334,67 @@ cudaError_t launch_xxh32_long(const uint8_t* base, const uint64_t* off, const in
 }
 #endif
 
+// xxh32_long_kernel (seed 0) for one run of a stream that goes on from call to call (the incremental frame writer): 64-bit
+// lengths, and the state carried in and out (XXH_CARRY_*).  The bytes of an unfinished stripe (a run that ends inside one,
+// after a flushed short block or a WRITE that stopped mid-stripe) wait in the state for the next run; a run that does not
+// complete the stripe only adds to them.
+__global__ void __launch_bounds__(32)
+xxh32_long_carry_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ off, const uint64_t* __restrict__ len,
+                        uint32_t* __restrict__ out, Xxh32Carry* __restrict__ c_state, const uint8_t* __restrict__ c_mode, uint32_t n)
+{
+    __shared__ __align__(16) uint8_t s_mem[16];
+    const uint32_t r = blockIdx.x;
+    if (r >= n) return;
+    const int lane = lane_id();
+    const uint32_t mode = c_mode[r];
+    const uint8_t* __restrict__ p = base + off[r];
+    uint64_t L = len[r];
+    uint32_t v = xxh32_chain_init(0u, lane), mem = 0;
+    uint64_t total = 0;
+    if (mode & XXH_CARRY_IN) {
+        const Xxh32Carry& c = c_state[r];
+        v = c.v[lane & 3]; total = c.total; mem = c.memsize;
+        if (uint32_t(lane) < mem) s_mem[lane] = c.mem[lane];
+    }
+    __syncwarp();
+    total += L;
+    if (mem + L < 16u) {                                    // the stripe stays open
+        if (uint32_t(lane) < L) s_mem[mem + lane] = p[lane];
+        mem += (uint32_t)L; L = 0;
+    } else {
+        if (mem) {                                          // finish the stripe the previous run left open
+            const uint32_t t = 16u - mem;
+            if (uint32_t(lane) < t) s_mem[mem + lane] = p[lane];
+            __syncwarp();
+            v = round32(v, reinterpret_cast<const uint32_t*>(s_mem)[lane & 3]);
+            p += t; L -= t; mem = 0;
+            __syncwarp();
+        }
+        const size_t stripes = size_t(L >> 4);
+        v = xxh32_warp_stripes(v, p, stripes, lane);
+        mem = uint32_t(L & 15u);
+        if (uint32_t(lane) < mem) s_mem[lane] = p[16 * stripes + lane];
+    }
+    __syncwarp();
+    if (mode & XXH_CARRY_OUT) {
+        Xxh32Carry& c = c_state[r];
+        if (lane < 4) c.v[lane] = v;
+        if (uint32_t(lane) < mem) c.mem[lane] = s_mem[lane];
+        if (lane == 0) { c.total = total; c.memsize = mem; }
+        return;
+    }
+    const uint32_t h = total >= 16 ? xxh32_chain_merge(v) : 0u + P32_5;
+    if (lane == 0) out[r] = finish32(h + uint32_t(total), s_mem, mem);
+}
+
+cudaError_t launch_xxh32_long_carry(const uint8_t* base, const uint64_t* off, const uint64_t* len, uint32_t* out, Xxh32Carry* carry,
+                                    const uint8_t* mode, size_t n, cudaStream_t st)
+{
+    if (n == 0) return cudaSuccess;
+    B200_LAUNCH(xxh32_long_carry_kernel, (unsigned)n, 32, st, base, off, len, out, carry, mode, (uint32_t)n);
+    return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------ frame content checksums, chained to the block decoder
 // LZ4FrameInputStream verifies a frame's content XXH32 after its last block (LZ4FrameInputStream.java:264-273).  As a
 // second pass over 32 frames of 64 MiB it costs as much as decoding them (a stream is four serial chains, ~3 GB/s, however

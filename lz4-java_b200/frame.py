@@ -230,6 +230,87 @@ class FrameReader:
             pass
 
 
+WRITE, FLUSH, CLOSE = 0, 1, 2
+
+
+class FrameWriter:
+    """ns LZ4 frame streams written piece by piece in device memory, each one LZ4FrameOutputStream whose content arrives over
+    time (b200lz4f_writer_*).  The writer is host data, the streams' carried state; not thread-safe.
+
+        with FrameWriter(ns, block_size_code=4) as wr:
+            status, consumed, produced, need = wr.write(src, src_off, src_len, out, dst_off, dst_cap, op)
+
+    A call writes stream s's header on its first call, then takes whole blocks from the start of its piece
+    src[src_off[s] : src_off[s] + src_len[s]]; op[s] FLUSH also takes the rest as a short block (flush()), CLOSE then writes the
+    EndMark and content checksum (close()).  The frame bytes go to out[dst_off[s] : dst_off[s] + produced[s]], never past
+    dst_cap[s].  The rest of the piece, past consumed[s], must start stream s's next piece.  status[s]: MORE_INPUT (need[s]:
+    the bytes missing for the next whole block), MORE_ROOM (need[s]: the room the next unit takes), DONE (latched).
+    known_size: the streams' declared content sizes (one int or one per stream; None: not declared).  src, out: contiguous
+    uint8 CUDA tensors on one device; the rest: host sequences.  Runs on torch's current stream and returns when the results
+    are on the host.  -> (status, consumed, produced, need): np.int32 / np.uint64 arrays."""
+
+    def __init__(self, ns: int, block_size_code: int = 4, content_checksum=True, block_checksum=False, known_size=None,
+                 hc_level: int = 0):
+        import ctypes
+        if not 4 <= block_size_code <= 7:
+            raise ValueError("block_size_code must be 4..7 (64 KiB .. 4 MiB)")
+        self.ns = int(ns)
+        flags = (1 if content_checksum else 0) | (2 if block_checksum else 0) | (4 if known_size is not None else 0)
+        known = None
+        if known_size is not None:
+            known = np.ascontiguousarray(np.broadcast_to(np.asarray(known_size, dtype=np.int64).reshape(-1), (self.ns,)))
+            if (known < 0).any():
+                raise ValueError("known_size must be >= 0")
+        err = ctypes.c_int(0)
+        self._h = N.lib().b200lz4f_writer_create(self.ns, block_size_code, flags, hc_level,
+                                                 known.ctypes.data if known is not None else None, ctypes.byref(err))
+        if not self._h:
+            N.check(err.value)
+            raise MemoryError("b200lz4f_writer_create")
+
+    def write(self, src, src_off, src_len, out, dst_off, dst_cap, op):
+        import torch
+        if not self._h:
+            raise ValueError("the writer is closed")
+        off, ln = _dev_streams(src, src_off, src_len, "piece")
+        if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+            raise ValueError("out must be a contiguous uint8 tensor on src's device")
+        doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+        dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+        ops = np.ascontiguousarray(np.asarray(op, dtype=np.int64).reshape(-1))
+        if len(ln) != self.ns or len(doff) != self.ns or len(dcap) != self.ns or len(ops) != self.ns:
+            raise ValueError(f"src_off, src_len, dst_off, dst_cap and op must have one entry per stream ({self.ns})")
+        if ((ops < WRITE) | (ops > CLOSE)).any():
+            raise ValueError("op must be WRITE, FLUSH or CLOSE")
+        if self.ns and int((doff + dcap).max()) > out.numel():
+            raise ValueError("a destination range reaches past the end of out")
+        ops = ops.astype(np.uint8)
+        status = np.zeros(self.ns, dtype=np.int32)
+        consumed, produced, need = (np.zeros(self.ns, dtype=np.uint64) for _ in range(3))
+        N.check(N.lib().b200lz4f_writer_write_dev(self._h, src.data_ptr(), off.ctypes.data, ln.ctypes.data, ops.ctypes.data,
+                                                  out.data_ptr(), doff.ctypes.data, dcap.ctypes.data, status.ctypes.data,
+                                                  consumed.ctypes.data, produced.ctypes.data, need.ctypes.data,
+                                                  torch.cuda.current_stream(src.device).cuda_stream))
+        return status, consumed, produced, need
+
+    def close(self):
+        if self._h:
+            N.lib().b200lz4f_writer_free(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ---- lz4-java's private "LZ4Block" container (LZ4BlockOutputStream / LZ4BlockInputStream)
 def compress_lz4block(src, block_size: int = 1 << 16, hc_level: int = 0) -> bytes:
     s = _view(src)
