@@ -308,6 +308,8 @@ int     b200lz4f_decompress_streams_dev(const uint8_t* d_src, const uint64_t* sr
  * byte.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep scratch
  * of the thread's context (the frame reader's segment buffers, record regions and decode slots), sized by the call -- the
  * pieces, the blocks taken, the room -- never by how long a stream has been read. */
+/* The statuses of the incremental frame calls, and of the incremental LZ4Block calls too (b200lz4block_writer_* /
+ * b200lz4block_reader_*) */
 #define B200LZ4F_MORE_INPUT 0
 #define B200LZ4F_MORE_ROOM  1
 #define B200LZ4F_DONE       2
@@ -359,6 +361,8 @@ int64_t b200lz4f_compress_dev(const uint8_t* d_src, const uint64_t* src_off, con
  * chunks, not on ns or the number of blocks; one synchronisation; only the plan, the ranges written and the checksum states
  * cross PCIe.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep
  * scratch of the thread's context (the frame writer's), sized by the call, never by how much a stream has written. */
+/* The ops of the incremental frame writer, and of the incremental LZ4Block writer too (b200lz4block_writer_*: FLUSH is
+ * flush() with syncFlush = true, CLOSE is finish() and its end block) */
 #define B200LZ4F_WRITE 0      /* take whole blocks only                                  */
 #define B200LZ4F_FLUSH 1      /* ... and the rest of the piece as a short block (flush()) */
 #define B200LZ4F_CLOSE 2      /* ... then the EndMark and content checksum (close())      */
@@ -419,6 +423,76 @@ int64_t b200lz4block_compress_dev(const uint8_t* d_src, const uint64_t* src_off,
 int     b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
                                     uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int stopOnEmptyBlock,
                                     int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream);
+/* Incremental device-resident LZ4Block writer for ns streams, each one LZ4BlockOutputStream(out, blockSize, compressor,
+ * XXHash32 seed 0x9747b28c, syncFlush) whose content arrives in pieces (LZ4BlockOutputStream.java:160-266): the incremental
+ * counterpart of b200lz4block_compress_dev, built from the same parts.  blockSize / hc_level as b200lz4block_compress_dev
+ * takes them, for every stream.  The ops and statuses are the frame calls': B200LZ4F_WRITE / _FLUSH / _CLOSE and
+ * B200LZ4F_MORE_INPUT / _MORE_ROOM / _DONE.  A writer (b200lz4block_writer_create) is host data, one byte of state per
+ * stream (whether it is closed); create and free make no CUDA call.  It returns NULL with *err = B200LZ4_E_ARG for a
+ * blockSize outside 64..32 MiB or ns above 2^31 - 1.  Any thread may use a writer, one at a time (it is not thread-safe,
+ * like LZ4BlockOutputStream).
+ * b200lz4block_writer_write_dev: stream s's next piece is src_len[s] bytes at d_src + src_off[s]; its stream bytes go to
+ * d_dst + dst_off[s] with room dst_cap[s]; op[s] is B200LZ4F_WRITE, _FLUSH or _CLOSE (HOST arrays of ns entries; the bytes
+ * device memory of the current device).  Per stream:
+ *  - The call takes whole blocks of blockSize from the start of the piece; with FLUSH (flush() with syncFlush = true) or
+ *    CLOSE (finish()) the rest of the piece as one short block (none when nothing is left); with CLOSE then the 21-byte
+ *    empty end block.
+ *  - A unit is taken only while the room left holds its bound: a block 21 + its length (a block that does not shrink is
+ *    stored), the end block 21.  The bytes go to [dst_off[s], dst_off[s] + produced[s]), never past dst_cap[s].
+ *  - src_consumed[s] is the bytes taken.  The rest of the piece is the caller's to present again at the start of the next
+ *    one: the writer keeps no payload byte between calls.
+ *  - status[s]: B200LZ4F_MORE_INPUT (need[s] = the bytes missing for the next whole block, blockSize after a flush),
+ *    B200LZ4F_MORE_ROOM (need[s] = the bound of the unit that did not fit), B200LZ4F_DONE (closed; latched: later calls
+ *    take and produce nothing).
+ *  - The concatenated output of stream s is byte for byte what LZ4BlockOutputStream writes for the same content with
+ *    syncFlush and flush() where FLUSH was passed, each block compressed by the library's block compressor at the 16-byte
+ *    phase where the call found it; with no FLUSH and pieces at the phase of the whole content, the stream
+ *    b200lz4block_compress_dev writes for it.
+ * Returns 0 or B200LZ4_E_*: a NULL writer or pointer, an op above _CLOSE, a destination range that overflows or more than
+ * 2^31 - 1 blocks in one call are found before anything is launched or written.  The launches depend on the number of
+ * chunks, not on ns or the number of blocks; one synchronisation; only the plan and the ranges written cross PCIe.  Ordered
+ * after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep scratch of the
+ * thread's context (the frame writer's), sized by the call, never by how much a stream has written. */
+void*   b200lz4block_writer_create(size_t ns, int blockSize, int hc_level, int* err);
+int     b200lz4block_writer_write_dev(void* writer, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                      const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                      int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream);
+void    b200lz4block_writer_free(void* writer);
+/* Incremental device-resident LZ4Block reader for ns streams, each one LZ4BlockInputStream(in, stopOnEmptyBlock) whose bytes
+ * arrive in pieces (LZ4BlockInputStream.java:191-264): the incremental counterpart of b200lz4block_decompress_dev, built from
+ * the same parts.  Statuses as for the frame calls (B200LZ4F_MORE_INPUT / _MORE_ROOM / _DONE).  A reader
+ * (b200lz4block_reader_create, ns above 2^31 - 1: NULL with *err = B200LZ4_E_ARG) is host data, the latched status of each
+ * stream; create and free make no CUDA call.  Any thread may use a reader, one at a time (it is not thread-safe, like
+ * LZ4BlockInputStream).
+ * b200lz4block_reader_read_dev: stream s's next piece is src_len[s] bytes at d_src + src_off[s]; its content goes to d_dst +
+ * dst_off[s] with room dst_cap[s]; eof[s] != 0 says the piece ends the stream (HOST arrays of ns entries; the bytes device
+ * memory of the current device).  Per stream:
+ *  - The call takes the complete units (a 21-byte block header with its payload) at the start of the piece, in stream
+ *    order, and decodes them straight into [dst_off[s], dst_off[s] + produced[s]).  It stops in front of the first unit the
+ *    piece holds only in part, and in front of the first block whose original length is above the room left: room is exact,
+ *    so there is no -9, and with dst_cap[s] >= the largest block every call with a complete unit progresses.
+ *    src_consumed[s] is where it stopped: the next piece must start at that byte of the stream.
+ *  - status[s]: B200LZ4F_MORE_INPUT (need[s] = the unit's length once its header is readable, else 21), B200LZ4F_MORE_ROOM
+ *    (need[s] = the block's original length), B200LZ4F_DONE (the first empty block with stopOnEmptyBlock; without it, eof
+ *    on a block boundary or inside a header, as LZ4BlockInputStream's tryReadFully ends quietly), or -1 / -2 as
+ *    b200lz4block_decompress_host returns them: an incomplete payload with eof is -1.  Errors come in stream order: the
+ *    blocks in front of the failing unit (a bad header, a failed decode or a wrong checksum) are delivered and counted in
+ *    produced[s], and src_consumed[s] is where the failing unit starts.  DONE and every error are latched: later calls
+ *    return the same status and take and produce nothing.
+ *  - After an error [dst_off[s] + produced[s], dst_off[s] + dst_cap[s]) holds unspecified bytes; nothing outside the
+ *    stream's range is ever written, and a call without an error writes nothing past produced[s].
+ *  - Whatever the pieces and room, the concatenated content, the final status and the total src_consumed are what
+ *    b200lz4block_decompress_host gives for the whole stream with ample room.
+ * Returns 0 or B200LZ4_E_*: a NULL reader or pointer, or a destination range that overflows are found before anything is
+ * launched.  The number of launches does not depend on ns or on the number of blocks; two synchronisations (scan totals,
+ * end); only the per-stream arguments, states and results and two totals cross to and from the host.  Ordered after the
+ * work already queued on `stream`; returns when the results are on the host.  Grow-or-keep scratch of the thread's context
+ * (the frame reader's segment buffers and record regions), sized by the call, never by how long a stream has been read. */
+void*   b200lz4block_reader_create(size_t ns, int stopOnEmptyBlock, int* err);
+int     b200lz4block_reader_read_dev(void* reader, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                     const uint8_t* eof, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                     int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream);
+void    b200lz4block_reader_free(void* reader);
 int     b200lz4_compress_with_length(const char* src, char* dst, int srcSize, int dstCapacity);
 int     b200lz4_decompressed_length(const char* src);
 int     b200lz4_decompress_with_length(const char* src, int srcAvail, char* dst, int dstCapacity);

@@ -12,12 +12,14 @@ from . import batch
 from . import frame
 from .frame import (decompress_frames, expected_content_size, compress_frame, compress_frames_dev, decompress_frames_dev,
                     decompress_frame_streams_dev, FrameReader, FrameWriter, compress_lz4block,
-                    decompress_lz4block, compress_lz4block_dev, decompress_lz4block_dev, compress_with_length, decompress_with_length,
+                    decompress_lz4block, compress_lz4block_dev, decompress_lz4block_dev, LZ4BlockWriter, LZ4BlockReader,
+                    compress_with_length, decompress_with_length,
                     compress_with_length_dev, decompress_with_length_dev, LZ4FrameError)
 
 __all__ = ["LZ4Factory", "LZ4Compressor", "LZ4FastDecompressor", "LZ4SafeDecompressor", "LZ4Exception",
            "XXHashFactory", "XXHash32", "XXHash64", "StreamingXXHash32", "StreamingXXHash64",
            "max_compressed_length", "batch", "B200Error", "frame", "decompress_frames", "compress_frame", "compress_frames_dev", "decompress_frames_dev",
            "decompress_frame_streams_dev", "FrameReader", "FrameWriter", "compress_lz4block",
-           "decompress_lz4block", "compress_lz4block_dev", "decompress_lz4block_dev", "expected_content_size", "compress_with_length",
+           "decompress_lz4block", "compress_lz4block_dev", "decompress_lz4block_dev", "LZ4BlockWriter", "LZ4BlockReader",
+           "expected_content_size", "compress_with_length",
            "decompress_with_length", "compress_with_length_dev", "decompress_with_length_dev", "LZ4FrameError"]

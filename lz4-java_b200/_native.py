@@ -92,6 +92,12 @@ SYMBOLS = [
     ("b200lz4block_decompress_host", C.c_int64, [_vp, _sz, _vp, _sz, C.c_int, _vp]),
     ("b200lz4block_compress_dev", C.c_int64, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _i, _i, _vp]),
     ("b200lz4block_decompress_dev", _i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    ("b200lz4block_writer_create", _vp, [_sz, _i, _i, _vp]),
+    ("b200lz4block_writer_write_dev", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    ("b200lz4block_writer_free", None, [_vp]),
+    ("b200lz4block_reader_create", _vp, [_sz, _i, _vp]),
+    ("b200lz4block_reader_read_dev", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    ("b200lz4block_reader_free", None, [_vp]),
     ("b200lz4_compress_with_length", _i, [_vp, _vp, _i, _i]),
     ("b200lz4_decompressed_length", _i, [_vp]),
     ("b200lz4_decompress_with_length", _i, [_vp, _i, _vp, _i]),

@@ -269,16 +269,19 @@ struct FrameWriterHandle {
     std::vector<FrameWriterState> st;
 };
 
-// What a call does for one stream, planned on the host from its piece's length, its op, its room and its state alone: the
-// header if it is due and fits, then whole blocks while their bounds fit, the short tail at FLUSH / CLOSE, the EndMark at
-// CLOSE.  mode: WRITER_* for the plan.
+// What a call does for one stream of an incremental writer, planned on the host from its piece's length, its op, its room
+// and its state alone: the header if it is due and fits, then whole blocks while their bounds fit, the short tail at
+// FLUSH / CLOSE, the stream's end at CLOSE.  The container's units: head the header's bytes (0: none due), word a block's
+// bytes besides its payload, tail the end's bytes -- a frame's header, block word (and checksum) and EndMark (and content
+// checksum); an LZ4Block stream's 21-byte block header and end block.  mode: WRITER_* for the plan.
 struct WriterTake { uint64_t taken, need; int32_t status; uint8_t mode; };
-static WriterTake writer_take(const FrameWriterState& w, uint64_t n, uint8_t op, uint64_t room, uint64_t bs, int flags)
+struct WriterUnits { uint64_t head, word, tail; };
+static WriterTake writer_take(bool done, uint64_t n, uint8_t op, uint64_t room, uint64_t bs, const WriterUnits& u)
 {
-    if (w.done) return { 0, 0, B200LZ4F_DONE, 0 };
-    const uint64_t head = 7 + ((flags & 4) ? 8 : 0), tail = 4 + ((flags & 1) ? 4 : 0), word = 4 + ((flags & 2) ? 4 : 0);
+    if (done) return { 0, 0, B200LZ4F_DONE, 0 };
+    const uint64_t head = u.head, tail = u.tail, word = u.word;
     WriterTake t{ 0, 0, B200LZ4F_MORE_ROOM, 0 };
-    if (!w.head) {                                                      // writeHeader (:178-191)
+    if (head) {                                                         // writeHeader (:178-191)
         if (room < head) { t.need = head; return t; }
         room -= head; t.mode |= WRITER_HEAD;
     }
@@ -325,7 +328,8 @@ static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, co
     std::vector<uint32_t> p_stream;
     uint64_t nb = 0, ni = 0, taken = 0;
     for (size_t k = 0; k < ns; k++) {
-        take[k] = writer_take(h->st[k], src_len[k], op[k], dst_cap[k], bs, flags);
+        const WriterUnits u{ h->st[k].head ? 0u : 7u + ((flags & 4) ? 8u : 0u), 4u + ((flags & 2) ? 4u : 0u), 4u + ((flags & 1) ? 4u : 0u) };
+        take[k] = writer_take(h->st[k].done, src_len[k], op[k], dst_cap[k], bs, u);
         if (!take[k].mode && !take[k].taken) continue;
         const uint64_t nbf = (take[k].taken + bs - 1) / bs;
         p_soff.push_back(src_off[k]); p_len.push_back(take[k].taken); p_stream.push_back((uint32_t)k);
@@ -397,6 +401,103 @@ static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, co
         if (take[k].status == B200LZ4F_DONE) h->st[k].done = 1;
     }
     for (size_t f = 0; f < xxh.size(); f++) h->st[p_stream[f]].xxh = xxh[f];
+    return 0;
+}
+
+// ---- the incremental LZ4Block writer (b200lz4block_writer_*; kernels: lz4block.cu).  The writer is host data: per stream
+// whether it is closed.
+struct Lz4BlockWriterHandle {
+    size_t ns; uint64_t bs; int level, hc_level;
+    std::vector<uint8_t> done;
+};
+
+// frame_writer_write_dev's steps with LZ4Block units (no header, 21 bytes per block, the 21-byte end block) and lz4block.cu's
+// writer kernels: the plan up, the checksums of the original blocks on the side stream from the start (as compress_blocks_dev
+// takes them), the chunks, the seal, each stream's range back, one synchronisation.
+static int lz4block_writer_write_dev(Lz4BlockWriterHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                     const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                     int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
+{
+    if (!h) return fail_arg("null writer");
+    const size_t ns = h->ns;
+    if (ns == 0) return 0;
+    if (!src_off || !src_len || !op || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
+        return fail_arg("null pointer");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+        if (op[k] > B200LZ4F_CLOSE) return fail_arg("op must be B200LZ4F_WRITE, _FLUSH or _CLOSE");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    const uint64_t bs = h->bs;
+    const WriterUnits units{ 0, LZ4BLOCK_HEADER, LZ4BLOCK_HEADER };
+    std::vector<WriterTake> take(ns);
+    std::vector<uint64_t> p_soff, p_len;
+    std::vector<uint32_t> p_stream;
+    uint64_t nb = 0, ni = 0, taken = 0;
+    for (size_t k = 0; k < ns; k++) {
+        take[k] = writer_take(h->done[k] != 0, src_len[k], op[k], dst_cap[k], bs, units);
+        if (!take[k].mode && !take[k].taken) continue;
+        const uint64_t nbf = (take[k].taken + bs - 1) / bs;
+        p_soff.push_back(src_off[k]); p_len.push_back(take[k].taken); p_stream.push_back((uint32_t)k);
+        nb += nbf; ni += nbf ? nbf : 1; taken += take[k].taken;
+    }
+    if (ni > 0x7FFFFFFFull) return fail_arg("more than 2^31 - 1 blocks in one call");
+    const size_t nf = p_stream.size();
+    std::vector<uint64_t> range(ns, 0);
+    if (nf) {
+        FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
+        const FramePlanLayout L(nb, ni, nf, nf);
+        rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
+        if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
+        if (rc) return rc;
+        uint8_t *H = s->h_plan, *D = s->d_plan;
+        std::vector<FrameChunk> chunks;
+        const uint64_t slots_need = plan_blocks(Container::LZ4Block, L, H, p_soff.data(), p_len.data(), nf, bs, chunks);
+        rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
+        for (size_t f = 0, i = 0; f < nf; f++) {
+            const size_t k = p_stream[f];
+            ((uint64_t*)(H + L.f_doff))[f] = dst_off[k];
+            ((uint32_t*)(H + L.f_first))[f] = (uint32_t)i;
+            (H + L.f_mode)[f] = take[k].mode;
+            ((uint64_t*)(H + L.f_known))[f] = 0;
+            i += p_len[f] ? (p_len[f] + bs - 1) / bs : 1;
+        }
+        const FramePlan P{ d_src, d_dst, s->d_slots,
+                           (const uint64_t*)(D + L.b_soff), (const int32_t*)(D + L.b_slen), (const uint64_t*)(D + L.b_slot), (const int32_t*)(D + L.b_clen),
+                           (uint64_t*)(D + L.b_poff), (int32_t*)(D + L.b_plen), (const uint32_t*)(D + L.b_sum),
+                           (const uint32_t*)(D + L.i_frame), (const int32_t*)(D + L.i_block), (int32_t*)(D + L.i_size), (uint64_t*)(D + L.i_off),
+                           (const uint64_t*)(D + L.f_len), (const uint32_t*)(D + L.f_sum), (uint64_t*)(D + L.f_off), (uint64_t*)(D + L.f_end),
+                           (uint32_t)ni, 0, 0, h->level };
+        const FrameWriterPlan W{ P, (const uint64_t*)(D + L.f_doff), (const uint32_t*)(D + L.f_first), (const uint8_t*)(D + L.f_mode) };
+
+        Drain drain{ st, side->st };
+        auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
+        CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
+        if (nb) {                   // the checksums of the original blocks, from the start, beside everything else
+            CK(cudaEventRecord(side->fork, st));
+            CK(cudaStreamWaitEvent(side->st, side->fork, 0));
+            CK(counted((taken / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+                d_src, P.b_soff, P.b_slen, LZ4BLOCK_SEED, (uint32_t*)P.b_sum, (size_t)nb, side->st)));
+            CK(cudaEventRecord(side->join, side->st));
+        }
+        rc = chunk_loop(P, (const int32_t*)(D + L.b_ccap), s->d_slots, chunks, h->hc_level, (uint64_t*)(D + L.carry),
+                        [&](uint32_t i0, uint32_t n) { return launch_lz4block_writer_sizes(W, i0, n, st); },
+                        [&](uint32_t i0, uint32_t n) { return launch_lz4block_writer_emit(W, i0, n, st); }, st);
+        if (rc) return rc;
+        if (nb) CK(cudaStreamWaitEvent(st, side->join, 0));
+        CK(counted(launch_lz4block_writer_seal(W, st)));
+        CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        drain.done = true;
+        for (size_t f = 0; f < nf; f++) range[p_stream[f]] = ((const uint64_t*)(H + L.f_end))[f] - ((const uint64_t*)(H + L.f_off))[f];
+    }
+    for (size_t k = 0; k < ns; k++) {
+        status[k] = take[k].status; src_consumed[k] = take[k].taken; produced[k] = range[k]; need[k] = take[k].need;
+        if (take[k].status == B200LZ4F_DONE) h->done[k] = 1;
+    }
     return 0;
 }
 
@@ -525,6 +626,120 @@ static int lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off
     memcpy(result, H + L.result, 8 * ns);
     if (src_consumed) memcpy(src_consumed, H + L.consumed, 8 * ns);
     if (content_len) memcpy(content_len, H + L.content, 8 * ns);
+    return 0;
+}
+
+// ---- the incremental LZ4Block reader (b200lz4block_reader_*; kernels: lz4block.cu).  The reader is host data: per stream
+// its latched status (0 while reading, B200LZ4F_DONE, or -1 / -2).
+struct Lz4BlockReaderHandle {
+    size_t ns; bool stop;
+    std::vector<int32_t> st;
+};
+// One call's per-stream arrays in the reader scratch's d_seg / h_seg: the arguments and states go up, the scan totals come
+// back after the counting walk, the results at the end.
+struct Lz4BlockReaderLayout {
+    size_t s_off, s_len, d_off, d_cap, eof, st_in, totals, n_comp, n_raw, tail, p_comp, p_raw, status, consumed, produced, need,
+           bytes = 0;
+    explicit Lz4BlockReaderLayout(size_t ns)
+    {
+        auto take = [&](size_t n) { const size_t at = bytes; bytes = (bytes + n + 15) & ~size_t(15); return at; };
+        s_off = take(8 * ns); s_len = take(8 * ns); d_off = take(8 * ns); d_cap = take(8 * ns); eof = take(ns); st_in = take(4 * ns);
+        totals = take(16);
+        n_comp = take(4 * ns); n_raw = take(4 * ns); tail = take(4 * ns); p_comp = take(8 * ns); p_raw = take(8 * ns);
+        status = take(4 * ns); consumed = take(8 * ns); produced = take(8 * ns); need = take(8 * ns);
+    }
+};
+
+// lz4block_decompress_dev's steps from each stream's latched status, with the walk resumable and the room applied by it:
+// counting walk, two scans (their totals come to the host, to size the records), recording walk, the blocks decode straight
+// into d_dst, their checksums, one verdict warp per stream.  The launches do not depend on the number of streams or blocks.
+static int lz4block_reader_read_dev(Lz4BlockReaderHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                    const uint8_t* eof, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                    int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
+{
+    if (!h) return fail_arg("null reader");
+    const size_t ns = h->ns;
+    if (ns == 0) return 0;
+    if (!src_off || !src_len || !eof || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
+        return fail_arg("null pointer");
+    uint64_t bytes = 0, room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    if (bytes / LZ4BLOCK_HEADER > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
+    FrameReadScratch* s;
+    int rc = get_frame_read_scratch(&s);
+    const Lz4BlockReaderLayout L(ns);
+    if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
+    if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
+    if (rc) return rc;
+    uint8_t *D = s->d_seg, *H = s->h_seg;
+    memcpy(H + L.s_off, src_off, 8 * ns); memcpy(H + L.s_len, src_len, 8 * ns);
+    memcpy(H + L.d_off, dst_off, 8 * ns); memcpy(H + L.d_cap, dst_cap, 8 * ns); memcpy(H + L.eof, eof, ns);
+    memcpy(H + L.st_in, h->st.data(), 4 * ns);
+    Lz4BlockReaderRead q{};
+    Lz4BlockRead& r = q.r;
+    r.src = d_src;
+    r.s_off = (const uint64_t*)(D + L.s_off); r.s_len = (const uint64_t*)(D + L.s_len);
+    r.d_off = (const uint64_t*)(D + L.d_off); r.d_cap = (const uint64_t*)(D + L.d_cap);
+    r.n_comp = (int32_t*)(D + L.n_comp); r.n_raw = (int32_t*)(D + L.n_raw); r.tail = (int32_t*)(D + L.tail);
+    r.p_comp = (const uint64_t*)(D + L.p_comp); r.p_raw = (const uint64_t*)(D + L.p_raw);
+    r.consumed = (uint64_t*)(D + L.consumed);
+    r.ns = (uint32_t)ns; r.stop = h->stop;
+    q.eof = D + L.eof; q.st_in = (const int32_t*)(D + L.st_in);
+    q.status = (int32_t*)(D + L.status); q.produced = (uint64_t*)(D + L.produced); q.need = (uint64_t*)(D + L.need);
+    uint64_t* totals = (uint64_t*)(D + L.totals);
+
+    Drain drain{ st };
+    CK(cudaMemcpyAsync(D, H, L.totals, cudaMemcpyHostToDevice, st));
+    g_launch_count.fetch_add(3, std::memory_order_relaxed);
+    CK(launch_lz4block_reader_walk(q, false, st));
+    CK(launch_scan(r.n_comp, (uint64_t*)r.p_comp, totals, nullptr, ns, st));
+    CK(launch_scan(r.n_raw, (uint64_t*)r.p_raw, totals + 1, nullptr, ns, st));
+    CK(cudaMemcpyAsync(H + L.totals, totals, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint64_t nc = ((const uint64_t*)(H + L.totals))[0], nr = ((const uint64_t*)(H + L.totals))[1], nb = nc + nr;
+    // the whole-stream reader's records, then per block where its unit starts
+    const Lz4BlockRecLayout R(nc, nr);
+    const size_t k_at = (R.bytes + 15) & ~size_t(15);
+    rc = reserve_device(s->d_recs, s->recs_cap, k_at + 8 * nb + 16); if (rc) return rc;
+    uint8_t* B = s->d_recs;
+    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
+    r.c_clen = (int32_t*)(B + R.c_clen); r.c_olen = (int32_t*)(B + R.c_olen); r.c_res = (int32_t*)(B + R.c_res);
+    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
+    r.b_doff = (uint64_t*)(B + R.b_doff); r.b_len = (int32_t*)(B + R.b_len); r.b_comp = (int32_t*)(B + R.b_comp);
+    r.b_want = (uint32_t*)(B + R.b_want); r.b_sum = (uint32_t*)(B + R.b_sum);
+    q.k_at = (uint64_t*)(B + k_at);
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
+    CK(launch_lz4block_reader_walk(q, true, st));
+    if (nr) {
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        CK(launch_gather(d_src, r.r_soff, r.r_len, d_dst, r.r_doff, (size_t)nr, st));
+    }
+    if (nc) {                       // as the host reader: src_avail = the compressed length, dst_len = the original length
+        const BatchArgs a{ d_src, r.c_soff, r.c_clen, d_dst, r.c_doff, r.c_olen, r.c_res, (size_t)nc };
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        CK(launch_decompress_fast(a, st));
+    }
+    if (nb) {                       // the decoded bytes are at most the room given, and at most 255 per source byte
+        const uint64_t decoded = room < bytes * 255 ? room : bytes * 255;
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        CK((decoded / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_dst, r.b_doff, r.b_len, LZ4BLOCK_SEED, r.b_sum, (size_t)nb, st));
+    }
+    g_launch_count.fetch_add(1, std::memory_order_relaxed);
+    CK(launch_lz4block_reader_verdict(q, st));
+    CK(cudaMemcpyAsync(H + L.status, D + L.status, L.bytes - L.status, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    drain.done = true;
+    memcpy(status, H + L.status, 4 * ns);
+    memcpy(src_consumed, H + L.consumed, 8 * ns);
+    memcpy(produced, H + L.produced, 8 * ns);
+    memcpy(need, H + L.need, 8 * ns);
+    for (size_t k = 0; k < ns; k++)
+        if (status[k] < 0 || status[k] == B200LZ4F_DONE) h->st[k] = status[k];
     return 0;
 }
 
@@ -740,6 +955,55 @@ int b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, c
     return b200::lz4block_decompress_dev(d_src, src_off, src_len, ns, d_dst, dst_off, dst_cap, stopOnEmptyBlock != 0, result,
                                          src_consumed, content_len, (cudaStream_t)stream);
 }
+
+// the incremental writer and reader (lz4block_writer_write_dev, lz4block_reader_read_dev): host data only, no CUDA call in
+// create or free
+void* b200lz4block_writer_create(size_t ns, int blockSize, int hc_level, int* err)
+{
+    if (err) *err = 0;
+    auto fail = [&](const char* what) -> void* { const int rc = b200::fail_arg(what); if (err) *err = rc; return nullptr; };
+    if (blockSize < 64 || blockSize > (1 << 25)) return fail("blockSize must be 64..32 MiB");
+    if (ns > 0x7FFFFFFFull) return fail("too many streams in one writer");
+    b200::Lz4BlockWriterHandle* h = new (std::nothrow) b200::Lz4BlockWriterHandle;
+    if (!h) return fail("out of host memory");
+    h->ns = ns; h->bs = (uint64_t)blockSize; h->level = b200::lz4block_level(blockSize); h->hc_level = hc_level;
+    try { h->done.assign(ns, 0); }
+    catch (...) { delete h; return fail("out of host memory"); }
+    return h;
+}
+
+int b200lz4block_writer_write_dev(void* writer, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                  const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                  int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream)
+{
+    return b200::lz4block_writer_write_dev((b200::Lz4BlockWriterHandle*)writer, d_src, src_off, src_len, op, d_dst, dst_off,
+                                           dst_cap, status, src_consumed, produced, need, (cudaStream_t)stream);
+}
+
+void b200lz4block_writer_free(void* writer) { delete (b200::Lz4BlockWriterHandle*)writer; }
+
+void* b200lz4block_reader_create(size_t ns, int stopOnEmptyBlock, int* err)
+{
+    if (err) *err = 0;
+    auto fail = [&](const char* what) -> void* { const int rc = b200::fail_arg(what); if (err) *err = rc; return nullptr; };
+    if (ns > 0x7FFFFFFFull) return fail("too many streams in one reader");
+    b200::Lz4BlockReaderHandle* h = new (std::nothrow) b200::Lz4BlockReaderHandle;
+    if (!h) return fail("out of host memory");
+    h->ns = ns; h->stop = stopOnEmptyBlock != 0;
+    try { h->st.assign(ns, 0); }
+    catch (...) { delete h; return fail("out of host memory"); }
+    return h;
+}
+
+int b200lz4block_reader_read_dev(void* reader, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                                 const uint8_t* eof, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                 int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream)
+{
+    return b200::lz4block_reader_read_dev((b200::Lz4BlockReaderHandle*)reader, d_src, src_off, src_len, eof, d_dst, dst_off,
+                                          dst_cap, status, src_consumed, produced, need, (cudaStream_t)stream);
+}
+
+void b200lz4block_reader_free(void* reader) { delete (b200::Lz4BlockReaderHandle*)reader; }
 
 // ---------------------------------------------------------------- length-prefixed block (LZ4CompressorWithLength.java:45-50)
 int b200lz4_compress_with_length(const char* src, char* dst, int srcSize, int dstCapacity)

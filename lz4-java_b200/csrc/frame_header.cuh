@@ -1,6 +1,6 @@
 // frame_header.cuh — what the two frame writers (frame_encode.cu, frame_writer.cu) write around the blocks: the header
 // (LZ4FrameOutputStream.writeHeader, LZ4FrameOutputStream.java:178-191), the block word's stored bit and the EndMark
-// (writeEndMark, :243-249).
+// (writeEndMark, :243-249); and the item placement both incremental writers (frame_writer.cu, lz4block.cu) share.
 #pragma once
 #include "common.cuh"
 #include "kernels.h"
@@ -13,6 +13,18 @@ __device__ __forceinline__ bool item_first(const FramePlan& p, uint32_t i) { ret
 __device__ __forceinline__ bool item_last(const FramePlan& p, uint32_t i) { return i + 1 == p.nitems || p.i_frame[i + 1] != p.i_frame[i]; }
 // stored as is when compression does not shrink the block (LZ4FrameOutputStream.java:215-222)
 __device__ __forceinline__ bool block_stored(int32_t clen, int32_t slen) { return clen <= 0 || clen >= slen; }
+
+// The incremental writers (frame_writer.cu, lz4block.cu): where item i lands, its stream's range then the bytes of the
+// stream's items before it in this call; whether it carries the stream's end (the EndMark, or the LZ4Block end block)
+__device__ __forceinline__ uint64_t writer_item_pos(const FrameWriterPlan& w, uint32_t i)
+{
+    const uint32_t f = w.p.i_frame[i];
+    return w.f_doff[f] + (w.p.i_off[i] - w.p.i_off[w.f_first[f]]);
+}
+__device__ __forceinline__ bool writer_tail(const FrameWriterPlan& w, uint32_t i)
+{
+    return (w.f_mode[w.p.i_frame[i]] & WRITER_TAIL) && item_last(w.p, i);
+}
 
 __device__ __forceinline__ void put_le32(uint8_t* p, uint32_t v)
 {

@@ -17,19 +17,9 @@
 
 namespace b200 {
 
-// where item i lands: its stream's range, then the bytes of the stream's items before it in this call
-__device__ __forceinline__ uint64_t writer_item_pos(const FrameWriterPlan& w, uint32_t i)
-{
-    const uint32_t f = w.p.i_frame[i];
-    return w.f_doff[f] + (w.p.i_off[i] - w.p.i_off[w.f_first[f]]);
-}
 __device__ __forceinline__ bool writer_head(const FrameWriterPlan& w, uint32_t i)
 {
     return (w.f_mode[w.p.i_frame[i]] & WRITER_HEAD) && item_first(w.p, i);
-}
-__device__ __forceinline__ bool writer_tail(const FrameWriterPlan& w, uint32_t i)
-{
-    return (w.f_mode[w.p.i_frame[i]] & WRITER_TAIL) && item_last(w.p, i);
 }
 
 // one thread per item of [i0, i0 + n)

@@ -349,21 +349,38 @@ cudaError_t launch_lz4block_sizes(const FramePlan& p, uint32_t i0, uint32_t n, c
 cudaError_t launch_lz4block_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
 // every item: block checksums (b_sum, masked to 28 bits), end blocks, f_off / f_end
 cudaError_t launch_lz4block_seal(const FramePlan& p, cudaStream_t st);
+// The incremental LZ4Block writer (b200lz4block_writer_*: lz4block_writer_write_dev in containers.cu): the incremental frame
+// writer's plan (FrameWriterPlan) with lz4block.cu's writer kernels.  No header is ever due; WRITER_TAIL puts the end block
+// on the plan frame's last item.
+cudaError_t launch_lz4block_writer_sizes(const FrameWriterPlan& w, uint32_t i0, uint32_t n, cudaStream_t st);
+cudaError_t launch_lz4block_writer_emit(const FrameWriterPlan& w, uint32_t i0, uint32_t n, cudaStream_t st);
+// every item: block checksums, end blocks, f_off / f_end as the stream's range written
+cudaError_t launch_lz4block_writer_seal(const FrameWriterPlan& w, cudaStream_t st);
 
 // The reader's walk of one stream, src[0, n), LZ4BlockInputStream.refill's header rules (:191-264).  Per block whose payload
 // is complete the sink gets block(payload offset, raw, compressed length, original length, checksum).  Returns where the walk
 // stopped and why: err 0 at the end of the stream (the first empty block with `stop`; without it, the end of src, quietly also
 // inside a header, :193-194), -1 premature end, -2 "Stream is corrupted".  Capacity is not the walk's: see Lz4BlockRoom.
-struct Lz4BlockEnd { uint64_t ip; int err; };
+//
+// walk_lz4block_from is the same walk, resumable (the incremental reader, lz4block.cu).  A unit is a 21-byte header with its
+// payload.  With `more` (bytes past n may come) a unit that src holds only in part is not an error: the walk stops in front
+// of it (stop WALK_STOP_INPUT, need = the unit's length once its header is readable, else 21).  A block whose original length
+// is above `room` stops it in front of that block (WALK_STOP_ROOM, need = that length); `room` is debited by each block
+// taken.  On an error ip is where the failing unit starts.  With `more` false and room ~0 it is walk_lz4block exactly.
+// walk_lz4block is the same code with Resumable false, so the whole-stream readers carry no room or input bookkeeping.
+struct Lz4BlockEnd { uint64_t ip; int err; uint8_t stop = WALK_STOP_NONE; uint64_t need = 0; };
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
-template <class Sink>
-__host__ __device__ inline Lz4BlockEnd walk_lz4block(const uint8_t* src, uint64_t n, bool stop, Sink& sink)
+template <bool Resumable, class Sink>
+__host__ __device__ inline Lz4BlockEnd walk_lz4block_impl(const uint8_t* src, uint64_t n, bool stop, bool more, uint64_t room, Sink& sink)
 {
     uint64_t ip = 0;
     for (;;) {
-        if (n - ip < (uint64_t)LZ4BLOCK_HEADER) return stop ? Lz4BlockEnd{ ip, -1 } : Lz4BlockEnd{ n, 0 };
+        if (n - ip < (uint64_t)LZ4BLOCK_HEADER) {
+            if (Resumable && more) return { ip, 0, WALK_STOP_INPUT, (uint64_t)LZ4BLOCK_HEADER };
+            return stop ? Lz4BlockEnd{ ip, -1 } : Lz4BlockEnd{ n, 0 };
+        }
         const uint8_t* h = src + ip;
         if (rd32(h) != LZ4BLOCK_MAGIC_LO || rd32(h + 4) != LZ4BLOCK_MAGIC_HI) return { ip, -2 };
         const int token = h[8], method = token & 0xF0, level = 10 + (token & 0x0F);
@@ -372,16 +389,40 @@ __host__ __device__ inline Lz4BlockEnd walk_lz4block(const uint8_t* src, uint64_
         const uint32_t check = rd32(h + 17);
         if (olen > (1 << level) || olen < 0 || clen < 0 || (olen == 0 && clen != 0) || (olen != 0 && clen == 0) ||
             (method == LZ4BLOCK_RAW && olen != clen)) return { ip, -2 };
+        const uint64_t unit = ip;
         ip += LZ4BLOCK_HEADER;
         if (olen == 0) {                                                        // empty block (:225-233)
-            if (check != 0) return { ip, -2 };
+            if (check != 0) return { Resumable ? unit : ip, -2 };
             if (stop) return { ip, 0 };
             continue;
         }
-        if (n - ip < (uint64_t)clen) return { ip, -1 };
+        if (n - ip < (uint64_t)clen) {
+            if (Resumable && more) return { unit, 0, WALK_STOP_INPUT, LZ4BLOCK_HEADER + (uint64_t)clen };
+            return { Resumable ? unit : ip, -1 };
+        }
+        if (Resumable) {
+            if ((uint64_t)olen > room) return { unit, 0, WALK_STOP_ROOM, (uint64_t)olen };
+            room -= (uint64_t)olen;
+        }
         sink.block(ip, method == LZ4BLOCK_RAW, clen, olen, check);
         ip += (uint64_t)clen;
     }
+}
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Sink>
+__host__ __device__ inline Lz4BlockEnd walk_lz4block_from(const uint8_t* src, uint64_t n, bool stop, bool more, uint64_t room, Sink& sink)
+{
+    return walk_lz4block_impl<true>(src, n, stop, more, room, sink);
+}
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Sink>
+__host__ __device__ inline Lz4BlockEnd walk_lz4block(const uint8_t* src, uint64_t n, bool stop, Sink& sink)
+{
+    return walk_lz4block_impl<false>(src, n, stop, false, ~0ull, sink);
 }
 // dst_cap applied behind the walk, the same way by both readers: blocks are taken while the prefix sum of their original
 // lengths fits; the first one that does not is the stream's -9 (unless a block before it fails its decode or checksum: -2).
@@ -413,6 +454,21 @@ struct Lz4BlockRead {
 cudaError_t launch_lz4block_walk(const Lz4BlockRead& r, bool record, cudaStream_t st);
 // one warp per stream: result, consumed
 cudaError_t launch_lz4block_verdict(const Lz4BlockRead& r, cudaStream_t st);
+
+// The incremental reader (b200lz4block_reader_*: lz4block_reader_read_dev in containers.cu, kernels in lz4block.cu), all
+// device pointers.  r holds the per-stream arguments and the block records as for b200lz4block_decompress_dev (r.consumed
+// is src_consumed; r.ip, r.content and r.result are unused).  Per stream its latched status (st_in: 0 while reading), the
+// results, and per block where its unit starts in the piece (k_at).
+struct Lz4BlockReaderRead {
+    Lz4BlockRead r;
+    const uint8_t* eof; const int32_t* st_in;
+    int32_t* status; uint64_t *produced, *need;
+    uint64_t* k_at;
+};
+// one thread per stream: with `record` false the counts, the walk's end in tail / consumed / need; with it every record
+cudaError_t launch_lz4block_reader_walk(const Lz4BlockReaderRead& q, bool record, cudaStream_t st);
+// one warp per stream: status, consumed, produced, need, cut at the first block that fails its decode or checksum
+cudaError_t launch_lz4block_reader_verdict(const Lz4BlockReaderRead& q, cudaStream_t st);
 
 // ---- length-prefixed records (LZ4CompressorWithLength / LZ4DecompressorWithLength).  The writer is the frame writer's loop
 // (compress_blocks_dev) with with_length.cu's item sizes and emit: a "frame" is one record, one item and one block of its

@@ -164,9 +164,67 @@ def decompress_frame_streams_dev(src, src_off, src_len, out, dst_off, dst_cap, r
 
 
 MORE_INPUT, MORE_ROOM, DONE = 0, 1, 2
+WRITE, FLUSH, CLOSE = 0, 1, 2
 
 
-class FrameReader:
+def _eofs(eof):
+    return np.ascontiguousarray(np.asarray(eof, dtype=bool).reshape(-1)).astype(np.uint8)
+
+
+def _ops(op):
+    return np.ascontiguousarray(np.asarray(op, dtype=np.int64).reshape(-1))
+
+
+class _Incremental:
+    """what the incremental readers and writers share: the argument checks of a call, the handle's lifetime (close(), the
+    context manager), torch's current stream.  _h: the handle; _free: the C call that frees it; _what: "reader" or "writer"."""
+    _h = None
+
+    def _call(self, fn, src, src_off, src_len, out, dst_off, dst_cap, last, last_name):
+        """last: eof or op, converted by _eofs or _ops; the checks run in the order FrameReader and FrameWriter always had"""
+        import torch
+        if not self._h:
+            raise ValueError(f"the {self._what} is closed")
+        off, ln = _dev_streams(src, src_off, src_len, "piece")
+        if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+            raise ValueError("out must be a contiguous uint8 tensor on src's device")
+        doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+        dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+        last = (_ops if last_name == "op" else _eofs)(last)
+        if len(ln) != self.ns or len(doff) != self.ns or len(dcap) != self.ns or len(last) != self.ns:
+            raise ValueError(f"src_off, src_len, dst_off, dst_cap and {last_name} must have one entry per stream ({self.ns})")
+        if last_name == "op":
+            if ((last < WRITE) | (last > CLOSE)).any():
+                raise ValueError("op must be WRITE, FLUSH or CLOSE")
+            last = last.astype(np.uint8)
+        if self.ns and int((doff + dcap).max()) > out.numel():
+            raise ValueError("a destination range reaches past the end of out")
+        status = np.zeros(self.ns, dtype=np.int32)
+        consumed, produced, need = (np.zeros(self.ns, dtype=np.uint64) for _ in range(3))
+        N.check(fn(self._h, src.data_ptr(), off.ctypes.data, ln.ctypes.data, last.ctypes.data, out.data_ptr(), doff.ctypes.data,
+                   dcap.ctypes.data, status.ctypes.data, consumed.ctypes.data, produced.ctypes.data, need.ctypes.data,
+                   torch.cuda.current_stream(src.device).cuda_stream))
+        return status, consumed, produced, need
+
+    def close(self):
+        if self._h:
+            getattr(N.lib(), self._free)(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class FrameReader(_Incremental):
     """ns LZ4 frame streams read piece by piece in device memory, each one LZ4FrameInputStream(in, readSingleFrame) whose
     bytes arrive over time (b200lz4f_reader_*).  The reader is host data, the streams' carried state; not thread-safe.
 
@@ -190,50 +248,13 @@ class FrameReader:
             N.check(err.value)
             raise MemoryError("b200lz4f_reader_create")
 
+    _free, _what = "b200lz4f_reader_free", "reader"
+
     def read(self, src, src_off, src_len, out, dst_off, dst_cap, eof):
-        import torch
-        if not self._h:
-            raise ValueError("the reader is closed")
-        off, ln = _dev_streams(src, src_off, src_len, "piece")
-        if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
-            raise ValueError("out must be a contiguous uint8 tensor on src's device")
-        doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
-        dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
-        end = np.ascontiguousarray(np.asarray(eof, dtype=bool).reshape(-1)).astype(np.uint8)
-        if len(ln) != self.ns or len(doff) != self.ns or len(dcap) != self.ns or len(end) != self.ns:
-            raise ValueError(f"src_off, src_len, dst_off, dst_cap and eof must have one entry per stream ({self.ns})")
-        if self.ns and int((doff + dcap).max()) > out.numel():
-            raise ValueError("a destination range reaches past the end of out")
-        status = np.zeros(self.ns, dtype=np.int32)
-        consumed, produced, need = (np.zeros(self.ns, dtype=np.uint64) for _ in range(3))
-        N.check(N.lib().b200lz4f_reader_read_dev(self._h, src.data_ptr(), off.ctypes.data, ln.ctypes.data, end.ctypes.data,
-                                                 out.data_ptr(), doff.ctypes.data, dcap.ctypes.data, status.ctypes.data,
-                                                 consumed.ctypes.data, produced.ctypes.data, need.ctypes.data,
-                                                 torch.cuda.current_stream(src.device).cuda_stream))
-        return status, consumed, produced, need
-
-    def close(self):
-        if self._h:
-            N.lib().b200lz4f_reader_free(self._h)
-            self._h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        return self._call(N.lib().b200lz4f_reader_read_dev, src, src_off, src_len, out, dst_off, dst_cap, eof, "eof")
 
 
-WRITE, FLUSH, CLOSE = 0, 1, 2
-
-
-class FrameWriter:
+class FrameWriter(_Incremental):
     """ns LZ4 frame streams written piece by piece in device memory, each one LZ4FrameOutputStream whose content arrives over
     time (b200lz4f_writer_*).  The writer is host data, the streams' carried state; not thread-safe.
 
@@ -268,47 +289,10 @@ class FrameWriter:
             N.check(err.value)
             raise MemoryError("b200lz4f_writer_create")
 
+    _free, _what = "b200lz4f_writer_free", "writer"
+
     def write(self, src, src_off, src_len, out, dst_off, dst_cap, op):
-        import torch
-        if not self._h:
-            raise ValueError("the writer is closed")
-        off, ln = _dev_streams(src, src_off, src_len, "piece")
-        if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
-            raise ValueError("out must be a contiguous uint8 tensor on src's device")
-        doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
-        dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
-        ops = np.ascontiguousarray(np.asarray(op, dtype=np.int64).reshape(-1))
-        if len(ln) != self.ns or len(doff) != self.ns or len(dcap) != self.ns or len(ops) != self.ns:
-            raise ValueError(f"src_off, src_len, dst_off, dst_cap and op must have one entry per stream ({self.ns})")
-        if ((ops < WRITE) | (ops > CLOSE)).any():
-            raise ValueError("op must be WRITE, FLUSH or CLOSE")
-        if self.ns and int((doff + dcap).max()) > out.numel():
-            raise ValueError("a destination range reaches past the end of out")
-        ops = ops.astype(np.uint8)
-        status = np.zeros(self.ns, dtype=np.int32)
-        consumed, produced, need = (np.zeros(self.ns, dtype=np.uint64) for _ in range(3))
-        N.check(N.lib().b200lz4f_writer_write_dev(self._h, src.data_ptr(), off.ctypes.data, ln.ctypes.data, ops.ctypes.data,
-                                                  out.data_ptr(), doff.ctypes.data, dcap.ctypes.data, status.ctypes.data,
-                                                  consumed.ctypes.data, produced.ctypes.data, need.ctypes.data,
-                                                  torch.cuda.current_stream(src.device).cuda_stream))
-        return status, consumed, produced, need
-
-    def close(self):
-        if self._h:
-            N.lib().b200lz4f_writer_free(self._h)
-            self._h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        return self._call(N.lib().b200lz4f_writer_write_dev, src, src_off, src_len, out, dst_off, dst_cap, op, "op")
 
 
 # ---- lz4-java's private "LZ4Block" container (LZ4BlockOutputStream / LZ4BlockInputStream)
@@ -404,6 +388,67 @@ def decompress_lz4block_dev(src, src_off, src_len, out, dst_off, dst_cap, stop_o
                                                 result.ctypes.data, consumed.ctypes.data, content.ctypes.data,
                                                 torch.cuda.current_stream(src.device).cuda_stream))
     return result, consumed, content
+
+
+class LZ4BlockWriter(_Incremental):
+    """ns LZ4Block streams written piece by piece in device memory, each one LZ4BlockOutputStream(out, blockSize, compressor,
+    checksum, syncFlush=True) whose content arrives over time (b200lz4block_writer_*).  The writer is host data, whether each
+    stream is closed; not thread-safe.
+
+        with LZ4BlockWriter(ns, block_size=1 << 16) as wr:
+            status, consumed, produced, need = wr.write(src, src_off, src_len, out, dst_off, dst_cap, op)
+
+    A call takes whole blocks from the start of stream s's piece src[src_off[s] : src_off[s] + src_len[s]]; op[s] FLUSH also
+    takes the rest as a short block (flush()), CLOSE then writes the empty end block (finish()).  The stream bytes go to
+    out[dst_off[s] : dst_off[s] + produced[s]], never past dst_cap[s].  The rest of the piece, past consumed[s], must start
+    stream s's next piece.  status[s]: MORE_INPUT (need[s]: the bytes missing for the next whole block), MORE_ROOM (need[s]:
+    the room the next unit takes, 21 + its length), DONE (latched).  hc_level 0: the fast compressor, 1..17: HC.  src, out:
+    contiguous uint8 CUDA tensors on one device; the rest: host sequences.  Runs on torch's current stream and returns when
+    the results are on the host.  -> (status, consumed, produced, need): np.int32 / np.uint64 arrays."""
+    _free, _what = "b200lz4block_writer_free", "writer"
+
+    def __init__(self, ns: int, block_size: int = 1 << 16, hc_level: int = 0):
+        import ctypes
+        if not 64 <= block_size <= 1 << 25:
+            raise ValueError("blockSize must be >= 64 and <= 32 MiB")            # LZ4BlockOutputStream.java:58-66
+        self.ns = int(ns)
+        err = ctypes.c_int(0)
+        self._h = N.lib().b200lz4block_writer_create(self.ns, block_size, hc_level, ctypes.byref(err))
+        if not self._h:
+            N.check(err.value)
+            raise MemoryError("b200lz4block_writer_create")
+
+    def write(self, src, src_off, src_len, out, dst_off, dst_cap, op):
+        return self._call(N.lib().b200lz4block_writer_write_dev, src, src_off, src_len, out, dst_off, dst_cap, op, "op")
+
+
+class LZ4BlockReader(_Incremental):
+    """ns LZ4Block streams read piece by piece in device memory, each one LZ4BlockInputStream(in, stopOnEmptyBlock) whose
+    bytes arrive over time (b200lz4block_reader_*).  The reader is host data, each stream's latched status; not thread-safe.
+
+        with LZ4BlockReader(ns) as rd:
+            status, consumed, produced, need = rd.read(src, src_off, src_len, out, dst_off, dst_cap, eof)
+
+    A call takes the complete blocks at the start of stream s's piece and decodes them into out[dst_off[s] : dst_off[s] +
+    produced[s]], never past dst_cap[s].  The next piece of stream s must start at byte consumed[s] of this one.  status[s]:
+    MORE_INPUT (need[s]: bytes the next unit takes), MORE_ROOM (need[s]: the next block's original length), DONE, or -1
+    (premature end) / -2 (corrupted), after the content in front of the failing unit was delivered.  eof[s] true: the piece
+    ends the stream.  DONE and errors are latched.  src, out: contiguous uint8 CUDA tensors on one device; the rest: host
+    sequences.  Runs on torch's current stream and returns when the results are on the host.  -> (status, consumed,
+    produced, need): np.int32 / np.uint64 arrays."""
+    _free, _what = "b200lz4block_reader_free", "reader"
+
+    def __init__(self, ns: int, stop_on_empty_block: bool = True):
+        import ctypes
+        err = ctypes.c_int(0)
+        self.ns = int(ns)
+        self._h = N.lib().b200lz4block_reader_create(self.ns, int(bool(stop_on_empty_block)), ctypes.byref(err))
+        if not self._h:
+            N.check(err.value)
+            raise MemoryError("b200lz4block_reader_create")
+
+    def read(self, src, src_off, src_len, out, dst_off, dst_cap, eof):
+        return self._call(N.lib().b200lz4block_reader_read_dev, src, src_off, src_len, out, dst_off, dst_cap, eof, "eof")
 
 
 # ---- LZ4CompressorWithLength / LZ4DecompressorWithLength
