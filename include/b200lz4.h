@@ -418,8 +418,9 @@ int64_t b200lz4block_compress_dev(const uint8_t* d_src, const uint64_t* src_off,
  * return -9.  On success nothing in d_dst outside [dst_off[s], dst_off[s] + result[s]) is written for stream s; on an error
  * [dst_off[s], dst_off[s] + dst_cap[s]) holds unspecified bytes and nothing outside it is written.  No payload byte crosses to
  * the host: per stream its arguments go up and its results come back, and two block counts in between.  Returns 0 or
- * B200LZ4_E_*.  Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep
- * scratch of the thread's context: the frame reader's. */
+ * B200LZ4_E_*: NULL pointers where bytes or results are needed, ns above 2^31 - 1 or a destination range that overflows are
+ * found before anything is launched.  Ordered after the work already queued on `stream`; returns when the results are on the
+ * host.  Grow-or-keep scratch of the thread's context: the frame reader's. */
 int     b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t ns,
                                     uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int stopOnEmptyBlock,
                                     int64_t* result, uint64_t* src_consumed, uint64_t* content_len, void* stream);
@@ -523,9 +524,10 @@ int64_t b200lz4_compress_with_length_dev(const uint8_t* d_src, const uint64_t* s
  * orig_len[r] (may be NULL): the declared length, -1 when src_len[r] < 4; a record refused for want of room can be read again
  * with dst_cap[r] = orig_len[r].  Nothing outside [dst_off[r], dst_off[r] + dst_cap[r]) is written, nothing at all for a
  * record its header rejects, and on success nothing past dst_off[r] + the declared length (fast) or + result[r] (safe).
- * Three launches whatever n is; only the per-record arguments go up and the results come back.  Returns 0 or B200LZ4_E_*.
- * Ordered after the work already queued on `stream`; returns when the results are on the host.  Grow-or-keep scratch of the
- * thread's context: the frame reader's. */
+ * Three launches whatever n is; only the per-record arguments go up and the results come back.  Returns 0 or B200LZ4_E_*:
+ * NULL pointers where bytes or results are needed, n above 2^31 - 1, a record above 2^31 - 1 bytes or a destination range
+ * that overflows are found before anything is launched.  Ordered after the work already queued on `stream`; returns when
+ * the results are on the host.  Grow-or-keep scratch of the thread's context: the frame reader's. */
 int     b200lz4_decompress_with_length_dev(const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, size_t n,
                                            uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, int safe,
                                            int64_t* result, int64_t* orig_len, void* stream);

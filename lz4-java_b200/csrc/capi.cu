@@ -35,6 +35,19 @@ int fail_cuda(cudaError_t e, const char* where)
 }
 int fail_arg(const char* what) { snprintf(tl_err, sizeof tl_err, "invalid argument: %s", what); return tl_status = B200LZ4_E_ARG; }
 
+int check_stream_ranges(size_t ns, const uint64_t* src_len, uint64_t src_max, const uint64_t* dst_off, const uint64_t* dst_cap,
+                        const void* d_src, const void* d_dst, uint64_t& bytes, uint64_t& room)
+{
+    bytes = 0; room = 0;
+    for (size_t k = 0; k < ns; k++) {
+        if (src_len[k] > src_max || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
+        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+        bytes += src_len[k]; room += dst_cap[k];
+    }
+    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    return 0;
+}
+
 static int ensure_device()
 {
     int cnt = 0;

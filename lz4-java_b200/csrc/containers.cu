@@ -125,7 +125,6 @@ template <class Sizes, class Emit>
 static int chunk_loop(const FramePlan& P, const int32_t* b_ccap, uint8_t* slots, const std::vector<FrameChunk>& chunks, int hc_level,
                       uint64_t* carry, Sizes sizes, Emit emit, cudaStream_t st)
 {
-    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     auto blocks = [&](size_t b0, size_t b1) {
         return BatchArgs{ P.src, P.b_soff + b0, P.b_slen + b0, slots, P.b_slot + b0, b_ccap + b0, (int32_t*)P.b_clen + b0, b1 - b0 };
     };
@@ -191,7 +190,6 @@ static int64_t compress_blocks_dev(Container kind, const uint8_t* d_src, const u
 
     // ---- launches, all ordered after what `st` already holds
     Drain drain{ st, side->st };
-    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
     // checksums of the sources alone, so from the start, beside everything else: the frame's content checksums, or the
     // LZ4Block checksums of the original blocks (records have none)
@@ -261,13 +259,28 @@ static int64_t compress_with_length_dev(const uint8_t* d_src, const uint64_t* sr
                                1ull << 31, 0, 0, hc_level, st);
 }
 
-// ---- the incremental frame writer (b200lz4f_writer_*; kernels: frame_writer.cu).  The writer is host data: the streams'
-// declared content sizes and one state each.
-struct FrameWriterHandle {
-    size_t ns; int bsCode, flags, hc_level;
+// ---- the incremental writers (b200lz4f_writer_*, b200lz4block_writer_*; kernels: frame_writer.cu, lz4block.cu).  A writer
+// is host data: the streams' declared content sizes (frames with flags bit 2) and one state each.  bs: bytes per block; code:
+// the frame's bsCode or the LZ4Block token's level nibble; flags: the frame's (0 for LZ4Block).
+struct WriterHandle {
+    Container kind; size_t ns; uint64_t bs; int code, flags, hc_level;
     std::vector<uint64_t> known;
     std::vector<FrameWriterState> st;
 };
+
+// A writer of ns streams with nothing written yet, or NULL when host memory runs out.  known: NULL, or ns declared sizes.
+static WriterHandle* new_writer(Container kind, size_t ns, uint64_t bs, int code, int flags, int hc_level, const int64_t* known)
+{
+    WriterHandle* h = new (std::nothrow) WriterHandle{ kind, ns, bs, code, flags, hc_level };
+    if (!h) return nullptr;
+    try {
+        if (known) h->known.assign((const uint64_t*)known, (const uint64_t*)known + ns);
+        FrameWriterState w{};                       // XXH32 with seed 0, nothing hashed yet (xxhash.c:445-455)
+        w.xxh.v[0] = 2654435761u + 2246822519u; w.xxh.v[1] = 2246822519u; w.xxh.v[2] = 0; w.xxh.v[3] = 0u - 2654435761u;
+        h->st.assign(ns, w);
+    } catch (...) { delete h; return nullptr; }
+    return h;
+}
 
 // What a call does for one stream of an incremental writer, planned on the host from its piece's length, its op, its room
 // and its state alone: the header if it is due and fits, then whole blocks while their bounds fit, the short tail at
@@ -301,34 +314,35 @@ static WriterTake writer_take(bool done, uint64_t n, uint8_t op, uint64_t room, 
     return t;
 }
 
-// compress_blocks_dev's plan and chunk loop over the streams that write something, with frame_writer.cu's item kernels: the
-// plan up, the carried content checksums on the side stream from the start, the chunks, the block checksums, the seal, each
-// stream's range and checksum state back, one synchronisation.
-static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
-                                  const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
-                                  int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
+// compress_blocks_dev's plan and chunk loop over the streams that write something, with the container's writer kernels: the
+// plan up, the early checksums on the side stream from the start (a frame's carried content checksums, or LZ4Block's checksums
+// of the original blocks), the chunks, the block checksums, the seal, each stream's range and checksum state back, one
+// synchronisation.
+static int writer_write_dev(WriterHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
+                            const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                            int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
 {
     if (!h) return fail_arg("null writer");
     const size_t ns = h->ns;
     if (ns == 0) return 0;
     if (!src_off || !src_len || !op || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
         return fail_arg("null pointer");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < ns; k++) {
-        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
-        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
+    uint64_t bytes, room;
+    int rc = check_stream_ranges(ns, src_len, 1ull << 47, dst_off, dst_cap, d_src, d_dst, bytes, room);
+    if (rc) return rc;
+    for (size_t k = 0; k < ns; k++)
         if (op[k] > B200LZ4F_CLOSE) return fail_arg("op must be B200LZ4F_WRITE, _FLUSH or _CLOSE");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    const bool frame = h->kind == Container::Frame;
     const int flags = h->flags;
-    const uint64_t bs = 1ull << (8 + 2 * h->bsCode);
+    const uint64_t bs = h->bs;
     std::vector<WriterTake> take(ns);
     std::vector<uint64_t> p_soff, p_len;
     std::vector<uint32_t> p_stream;
     uint64_t nb = 0, ni = 0, taken = 0;
     for (size_t k = 0; k < ns; k++) {
-        const WriterUnits u{ h->st[k].head ? 0u : 7u + ((flags & 4) ? 8u : 0u), 4u + ((flags & 2) ? 4u : 0u), 4u + ((flags & 1) ? 4u : 0u) };
+        const WriterUnits u = frame ? WriterUnits{ h->st[k].head ? 0u : 7u + ((flags & 4) ? 8u : 0u), 4u + ((flags & 2) ? 4u : 0u),
+                                                   4u + ((flags & 1) ? 4u : 0u) }
+                                    : WriterUnits{ 0, LZ4BLOCK_HEADER, LZ4BLOCK_HEADER };
         take[k] = writer_take(h->st[k].done, src_len[k], op[k], dst_cap[k], bs, u);
         if (!take[k].mode && !take[k].taken) continue;
         const uint64_t nbf = (take[k].taken + bs - 1) / bs;
@@ -340,14 +354,14 @@ static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, co
     std::vector<uint64_t> range(ns, 0);
     std::vector<Xxh32Carry> xxh;
     if (nf) {
-        FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
+        FrameScratch* s; SideStream* side; rc = get_frame_scratch(&s, &side); if (rc) return rc;
         const FramePlanLayout L(nb, ni, nf, nf, nx);
         rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
         if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
         if (rc) return rc;
         uint8_t *H = s->h_plan, *D = s->d_plan;
         std::vector<FrameChunk> chunks;
-        const uint64_t slots_need = plan_blocks(Container::Frame, L, H, p_soff.data(), p_len.data(), nf, bs, chunks);
+        const uint64_t slots_need = plan_blocks(h->kind, L, H, p_soff.data(), p_len.data(), nf, bs, chunks);
         rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
         for (size_t f = 0, i = 0; f < nf; f++) {
             const size_t k = p_stream[f];
@@ -361,34 +375,41 @@ static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, co
             }
             i += p_len[f] ? (p_len[f] + bs - 1) / bs : 1;
         }
+        // p.f_len is the declared content size; the LZ4Block writer kernels do not read it
         const FramePlan P{ d_src, d_dst, s->d_slots,
                            (const uint64_t*)(D + L.b_soff), (const int32_t*)(D + L.b_slen), (const uint64_t*)(D + L.b_slot), (const int32_t*)(D + L.b_clen),
                            (uint64_t*)(D + L.b_poff), (int32_t*)(D + L.b_plen), (const uint32_t*)(D + L.b_sum),
                            (const uint32_t*)(D + L.i_frame), (const int32_t*)(D + L.i_block), (int32_t*)(D + L.i_size), (uint64_t*)(D + L.i_off),
                            (const uint64_t*)(D + L.f_known), (const uint32_t*)(D + L.f_sum), (uint64_t*)(D + L.f_off), (uint64_t*)(D + L.f_end),
-                           (uint32_t)ni, h->bsCode, flags, 0 };
+                           (uint32_t)ni, frame ? h->code : 0, flags, frame ? 0 : h->code };
         const FrameWriterPlan W{ P, (const uint64_t*)(D + L.f_doff), (const uint32_t*)(D + L.f_first), (const uint8_t*)(D + L.f_mode) };
 
         Drain drain{ st, side->st };
-        auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
         CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
-        if (nx) {                   // the content checksums of the runs taken, from the start, beside everything else
+        const bool early_sums = frame ? nx != 0 : nb > 0;
+        if (early_sums) {           // checksums of the sources alone, so from the start, beside everything else
             CK(cudaEventRecord(side->fork, st));
             CK(cudaStreamWaitEvent(side->st, side->fork, 0));
-            CK(counted(launch_xxh32_long_carry(d_src, (const uint64_t*)(D + L.f_soff), (const uint64_t*)(D + L.f_len),
-                                               (uint32_t*)(D + L.f_sum), (Xxh32Carry*)(D + L.f_xxh), D + L.f_xmode, nf, side->st)));
+            if (frame)
+                CK(counted(launch_xxh32_long_carry(d_src, (const uint64_t*)(D + L.f_soff), (const uint64_t*)(D + L.f_len),
+                                                   (uint32_t*)(D + L.f_sum), (Xxh32Carry*)(D + L.f_xxh), D + L.f_xmode, nf, side->st)));
+            else
+                CK(counted((taken / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
+                    d_src, P.b_soff, P.b_slen, LZ4BLOCK_SEED, (uint32_t*)P.b_sum, (size_t)nb, side->st)));
             CK(cudaEventRecord(side->join, side->st));
         }
         rc = chunk_loop(P, (const int32_t*)(D + L.b_ccap), s->d_slots, chunks, h->hc_level, (uint64_t*)(D + L.carry),
-                        [&](uint32_t i0, uint32_t n) { return launch_frame_writer_sizes(W, i0, n, st); },
-                        [&](uint32_t i0, uint32_t n) { return launch_frame_writer_emit(W, i0, n, st); }, st);
+                        [&](uint32_t i0, uint32_t n) { return frame ? launch_frame_writer_sizes(W, i0, n, st)
+                                                                     : launch_lz4block_writer_sizes(W, i0, n, st); },
+                        [&](uint32_t i0, uint32_t n) { return frame ? launch_frame_writer_emit(W, i0, n, st)
+                                                                     : launch_lz4block_writer_emit(W, i0, n, st); }, st);
         if (rc) return rc;
         if ((flags & 2) && nb) {    // block checksums over the payloads as written, as compress_blocks_dev takes them
             CK(counted((taken / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
                 d_dst, P.b_poff, P.b_plen, 0, (uint32_t*)P.b_sum, (size_t)nb, st)));
         }
-        if (nx) CK(cudaStreamWaitEvent(st, side->join, 0));
-        CK(counted(launch_frame_writer_seal(W, st)));
+        if (early_sums) CK(cudaStreamWaitEvent(st, side->join, 0));
+        CK(counted(frame ? launch_frame_writer_seal(W, st) : launch_lz4block_writer_seal(W, st)));
         CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         drain.done = true;
@@ -401,103 +422,6 @@ static int frame_writer_write_dev(FrameWriterHandle* h, const uint8_t* d_src, co
         if (take[k].status == B200LZ4F_DONE) h->st[k].done = 1;
     }
     for (size_t f = 0; f < xxh.size(); f++) h->st[p_stream[f]].xxh = xxh[f];
-    return 0;
-}
-
-// ---- the incremental LZ4Block writer (b200lz4block_writer_*; kernels: lz4block.cu).  The writer is host data: per stream
-// whether it is closed.
-struct Lz4BlockWriterHandle {
-    size_t ns; uint64_t bs; int level, hc_level;
-    std::vector<uint8_t> done;
-};
-
-// frame_writer_write_dev's steps with LZ4Block units (no header, 21 bytes per block, the 21-byte end block) and lz4block.cu's
-// writer kernels: the plan up, the checksums of the original blocks on the side stream from the start (as compress_blocks_dev
-// takes them), the chunks, the seal, each stream's range back, one synchronisation.
-static int lz4block_writer_write_dev(Lz4BlockWriterHandle* h, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
-                                     const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
-                                     int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, cudaStream_t st)
-{
-    if (!h) return fail_arg("null writer");
-    const size_t ns = h->ns;
-    if (ns == 0) return 0;
-    if (!src_off || !src_len || !op || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
-        return fail_arg("null pointer");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < ns; k++) {
-        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
-        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
-        if (op[k] > B200LZ4F_CLOSE) return fail_arg("op must be B200LZ4F_WRITE, _FLUSH or _CLOSE");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
-    const uint64_t bs = h->bs;
-    const WriterUnits units{ 0, LZ4BLOCK_HEADER, LZ4BLOCK_HEADER };
-    std::vector<WriterTake> take(ns);
-    std::vector<uint64_t> p_soff, p_len;
-    std::vector<uint32_t> p_stream;
-    uint64_t nb = 0, ni = 0, taken = 0;
-    for (size_t k = 0; k < ns; k++) {
-        take[k] = writer_take(h->done[k] != 0, src_len[k], op[k], dst_cap[k], bs, units);
-        if (!take[k].mode && !take[k].taken) continue;
-        const uint64_t nbf = (take[k].taken + bs - 1) / bs;
-        p_soff.push_back(src_off[k]); p_len.push_back(take[k].taken); p_stream.push_back((uint32_t)k);
-        nb += nbf; ni += nbf ? nbf : 1; taken += take[k].taken;
-    }
-    if (ni > 0x7FFFFFFFull) return fail_arg("more than 2^31 - 1 blocks in one call");
-    const size_t nf = p_stream.size();
-    std::vector<uint64_t> range(ns, 0);
-    if (nf) {
-        FrameScratch* s; SideStream* side; int rc = get_frame_scratch(&s, &side); if (rc) return rc;
-        const FramePlanLayout L(nb, ni, nf, nf);
-        rc = reserve_pinned(s->h_plan, s->h_plan_cap, L.bytes);
-        if (!rc) rc = reserve_device(s->d_plan, s->plan_cap, L.bytes);
-        if (rc) return rc;
-        uint8_t *H = s->h_plan, *D = s->d_plan;
-        std::vector<FrameChunk> chunks;
-        const uint64_t slots_need = plan_blocks(Container::LZ4Block, L, H, p_soff.data(), p_len.data(), nf, bs, chunks);
-        rc = reserve_device(s->d_slots, s->slots_cap, (size_t)slots_need + 16); if (rc) return rc;
-        for (size_t f = 0, i = 0; f < nf; f++) {
-            const size_t k = p_stream[f];
-            ((uint64_t*)(H + L.f_doff))[f] = dst_off[k];
-            ((uint32_t*)(H + L.f_first))[f] = (uint32_t)i;
-            (H + L.f_mode)[f] = take[k].mode;
-            ((uint64_t*)(H + L.f_known))[f] = 0;
-            i += p_len[f] ? (p_len[f] + bs - 1) / bs : 1;
-        }
-        const FramePlan P{ d_src, d_dst, s->d_slots,
-                           (const uint64_t*)(D + L.b_soff), (const int32_t*)(D + L.b_slen), (const uint64_t*)(D + L.b_slot), (const int32_t*)(D + L.b_clen),
-                           (uint64_t*)(D + L.b_poff), (int32_t*)(D + L.b_plen), (const uint32_t*)(D + L.b_sum),
-                           (const uint32_t*)(D + L.i_frame), (const int32_t*)(D + L.i_block), (int32_t*)(D + L.i_size), (uint64_t*)(D + L.i_off),
-                           (const uint64_t*)(D + L.f_len), (const uint32_t*)(D + L.f_sum), (uint64_t*)(D + L.f_off), (uint64_t*)(D + L.f_end),
-                           (uint32_t)ni, 0, 0, h->level };
-        const FrameWriterPlan W{ P, (const uint64_t*)(D + L.f_doff), (const uint32_t*)(D + L.f_first), (const uint8_t*)(D + L.f_mode) };
-
-        Drain drain{ st, side->st };
-        auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
-        CK(cudaMemcpyAsync(D, H, L.bytes, cudaMemcpyHostToDevice, st));
-        if (nb) {                   // the checksums of the original blocks, from the start, beside everything else
-            CK(cudaEventRecord(side->fork, st));
-            CK(cudaStreamWaitEvent(side->st, side->fork, 0));
-            CK(counted((taken / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(
-                d_src, P.b_soff, P.b_slen, LZ4BLOCK_SEED, (uint32_t*)P.b_sum, (size_t)nb, side->st)));
-            CK(cudaEventRecord(side->join, side->st));
-        }
-        rc = chunk_loop(P, (const int32_t*)(D + L.b_ccap), s->d_slots, chunks, h->hc_level, (uint64_t*)(D + L.carry),
-                        [&](uint32_t i0, uint32_t n) { return launch_lz4block_writer_sizes(W, i0, n, st); },
-                        [&](uint32_t i0, uint32_t n) { return launch_lz4block_writer_emit(W, i0, n, st); }, st);
-        if (rc) return rc;
-        if (nb) CK(cudaStreamWaitEvent(st, side->join, 0));
-        CK(counted(launch_lz4block_writer_seal(W, st)));
-        CK(cudaMemcpyAsync(H + L.f_off, D + L.f_off, L.bytes - L.f_off, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        drain.done = true;
-        for (size_t f = 0; f < nf; f++) range[p_stream[f]] = ((const uint64_t*)(H + L.f_end))[f] - ((const uint64_t*)(H + L.f_off))[f];
-    }
-    for (size_t k = 0; k < ns; k++) {
-        status[k] = take[k].status; src_consumed[k] = take[k].taken; produced[k] = range[k]; need[k] = take[k].need;
-        if (take[k].status == B200LZ4F_DONE) h->done[k] = 1;
-    }
     return 0;
 }
 
@@ -548,6 +472,36 @@ struct Lz4BlockRecLayout {
     }
 };
 
+// Points r's record arrays into the call's record region B.
+static void bind_lz4block_records(Lz4BlockRead& r, uint8_t* B, const Lz4BlockRecLayout& R)
+{
+    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
+    r.c_clen = (int32_t*)(B + R.c_clen); r.c_olen = (int32_t*)(B + R.c_olen); r.c_res = (int32_t*)(B + R.c_res);
+    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
+    r.b_doff = (uint64_t*)(B + R.b_doff); r.b_len = (int32_t*)(B + R.b_len); r.b_comp = (int32_t*)(B + R.b_comp);
+    r.b_want = (uint32_t*)(B + R.b_want); r.b_sum = (uint32_t*)(B + R.b_sum);
+}
+
+// The payload launches behind a recording walk: the stored blocks gathered and the compressed ones decoded straight into
+// d_dst, then the XXH32 of every decoded block.  bytes / room: the call's source bytes and room; nc / nr: its compressed /
+// stored blocks.
+static int lz4block_payload_launches(const Lz4BlockRead& r, uint8_t* d_dst, uint64_t bytes, uint64_t room, uint64_t nc,
+                                     uint64_t nr, cudaStream_t st)
+{
+    const uint64_t nb = nc + nr;
+    if (nr) CK(counted(launch_gather(r.src, r.r_soff, r.r_len, d_dst, r.r_doff, (size_t)nr, st)));
+    if (nc) {                       // as the host reader: src_avail = the compressed length, dst_len = the original length
+        const BatchArgs a{ r.src, r.c_soff, r.c_clen, d_dst, r.c_doff, r.c_olen, r.c_res, (size_t)nc };
+        CK(counted(launch_decompress_fast(a, st)));
+    }
+    if (nb) {                       // the decoded bytes are at most the room given, and at most 255 per source byte
+        const uint64_t decoded = room < bytes * 255 ? room : bytes * 255;
+        CK(counted((decoded / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_dst, r.b_doff, r.b_len, LZ4BLOCK_SEED,
+                                                                                      r.b_sum, (size_t)nb, st)));
+    }
+    return 0;
+}
+
 // Counting walk, two scans of the counts (only their totals come to the host: the records' room), recording walk, then
 // the blocks decode straight into d_dst, their checksums, and one verdict per stream.  The launches do not depend on the
 // number of streams or blocks.
@@ -558,15 +512,12 @@ static int lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off
     if (ns == 0) return 0;
     if (!src_off || !src_len || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
     if (ns > 0x7FFFFFFFull) return fail_arg("too many streams in one call");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < ns; k++) {
-        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    uint64_t bytes, room;
+    int rc = check_stream_ranges(ns, src_len, 1ull << 47, dst_off, dst_cap, d_src, d_dst, bytes, room);
+    if (rc) return rc;
     if (bytes / LZ4BLOCK_HEADER > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
     FrameReadScratch* s;
-    int rc = get_frame_read_scratch(&s);
+    rc = get_frame_read_scratch(&s);
     const Lz4BlockStreamLayout L(ns);
     if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
     if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
@@ -593,33 +544,13 @@ static int lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off
     CK(launch_scan(r.n_raw, (uint64_t*)r.p_raw, totals + 1, nullptr, ns, st));
     CK(cudaMemcpyAsync(H + L.totals, totals, 16, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    const uint64_t nc = ((const uint64_t*)(H + L.totals))[0], nr = ((const uint64_t*)(H + L.totals))[1], nb = nc + nr;
+    const uint64_t nc = ((const uint64_t*)(H + L.totals))[0], nr = ((const uint64_t*)(H + L.totals))[1];
     const Lz4BlockRecLayout R(nc, nr);
     rc = reserve_device(s->d_recs, s->recs_cap, R.bytes + 16); if (rc) return rc;
-    uint8_t* B = s->d_recs;
-    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
-    r.c_clen = (int32_t*)(B + R.c_clen); r.c_olen = (int32_t*)(B + R.c_olen); r.c_res = (int32_t*)(B + R.c_res);
-    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
-    r.b_doff = (uint64_t*)(B + R.b_doff); r.b_len = (int32_t*)(B + R.b_len); r.b_comp = (int32_t*)(B + R.b_comp);
-    r.b_want = (uint32_t*)(B + R.b_want); r.b_sum = (uint32_t*)(B + R.b_sum);
-    g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    CK(launch_lz4block_walk(r, true, st));
-    if (nr) {
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        CK(launch_gather(d_src, r.r_soff, r.r_len, d_dst, r.r_doff, (size_t)nr, st));
-    }
-    if (nc) {                       // as the host reader: src_avail = the compressed length, dst_len = the original length
-        const BatchArgs a{ d_src, r.c_soff, r.c_clen, d_dst, r.c_doff, r.c_olen, r.c_res, (size_t)nc };
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        CK(launch_decompress_fast(a, st));
-    }
-    if (nb) {                       // the decoded bytes are at most the room given, and at most 255 per source byte
-        const uint64_t decoded = room < bytes * 255 ? room : bytes * 255;
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        CK((decoded / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_dst, r.b_doff, r.b_len, LZ4BLOCK_SEED, r.b_sum, (size_t)nb, st));
-    }
-    g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    CK(launch_lz4block_verdict(r, st));
+    bind_lz4block_records(r, s->d_recs, R);
+    CK(counted(launch_lz4block_walk(r, true, st)));
+    rc = lz4block_payload_launches(r, d_dst, bytes, room, nc, nr, st); if (rc) return rc;
+    CK(counted(launch_lz4block_verdict(r, st)));
     CK(cudaMemcpyAsync(H + L.result, D + L.result, L.bytes - L.result, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     drain.done = true;
@@ -662,16 +593,12 @@ static int lz4block_reader_read_dev(Lz4BlockReaderHandle* h, const uint8_t* d_sr
     if (ns == 0) return 0;
     if (!src_off || !src_len || !eof || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
         return fail_arg("null pointer");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < ns; k++) {
-        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
-        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    uint64_t bytes, room;
+    int rc = check_stream_ranges(ns, src_len, 1ull << 47, dst_off, dst_cap, d_src, d_dst, bytes, room);
+    if (rc) return rc;
     if (bytes / LZ4BLOCK_HEADER > 0x7FFFFFFFull) return fail_arg("too many blocks in one call");
     FrameReadScratch* s;
-    int rc = get_frame_read_scratch(&s);
+    rc = get_frame_read_scratch(&s);
     const Lz4BlockReaderLayout L(ns);
     if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
     if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
@@ -706,31 +633,11 @@ static int lz4block_reader_read_dev(Lz4BlockReaderHandle* h, const uint8_t* d_sr
     const Lz4BlockRecLayout R(nc, nr);
     const size_t k_at = (R.bytes + 15) & ~size_t(15);
     rc = reserve_device(s->d_recs, s->recs_cap, k_at + 8 * nb + 16); if (rc) return rc;
-    uint8_t* B = s->d_recs;
-    r.c_soff = (uint64_t*)(B + R.c_soff); r.c_doff = (uint64_t*)(B + R.c_doff);
-    r.c_clen = (int32_t*)(B + R.c_clen); r.c_olen = (int32_t*)(B + R.c_olen); r.c_res = (int32_t*)(B + R.c_res);
-    r.r_soff = (uint64_t*)(B + R.r_soff); r.r_doff = (uint64_t*)(B + R.r_doff); r.r_len = (int32_t*)(B + R.r_len);
-    r.b_doff = (uint64_t*)(B + R.b_doff); r.b_len = (int32_t*)(B + R.b_len); r.b_comp = (int32_t*)(B + R.b_comp);
-    r.b_want = (uint32_t*)(B + R.b_want); r.b_sum = (uint32_t*)(B + R.b_sum);
-    q.k_at = (uint64_t*)(B + k_at);
-    g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    CK(launch_lz4block_reader_walk(q, true, st));
-    if (nr) {
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        CK(launch_gather(d_src, r.r_soff, r.r_len, d_dst, r.r_doff, (size_t)nr, st));
-    }
-    if (nc) {                       // as the host reader: src_avail = the compressed length, dst_len = the original length
-        const BatchArgs a{ d_src, r.c_soff, r.c_clen, d_dst, r.c_doff, r.c_olen, r.c_res, (size_t)nc };
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        CK(launch_decompress_fast(a, st));
-    }
-    if (nb) {                       // the decoded bytes are at most the room given, and at most 255 per source byte
-        const uint64_t decoded = room < bytes * 255 ? room : bytes * 255;
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        CK((decoded / nb >= XXH_LONG_AVG ? launch_xxh32_long : launch_xxh32)(d_dst, r.b_doff, r.b_len, LZ4BLOCK_SEED, r.b_sum, (size_t)nb, st));
-    }
-    g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    CK(launch_lz4block_reader_verdict(q, st));
+    bind_lz4block_records(r, s->d_recs, R);
+    q.k_at = (uint64_t*)(s->d_recs + k_at);
+    CK(counted(launch_lz4block_reader_walk(q, true, st)));
+    rc = lz4block_payload_launches(r, d_dst, bytes, room, nc, nr, st); if (rc) return rc;
+    CK(counted(launch_lz4block_reader_verdict(q, st)));
     CK(cudaMemcpyAsync(H + L.status, D + L.status, L.bytes - L.status, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     drain.done = true;
@@ -766,15 +673,11 @@ static int with_length_decompress_dev(const uint8_t* d_src, const uint64_t* src_
     if (n == 0) return 0;
     if (!src_off || !src_len || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
     if (n > 0x7FFFFFFFull) return fail_arg("too many records in one call");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < n; k++) {
-        if (src_len[k] > 0x7FFFFFFFull) return fail_arg("src_len: a record is at most 2^31 - 1 bytes");
-        if (dst_cap[k] > (1ull << 47)) return fail_arg("dst_cap");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    uint64_t bytes, room;                                           // a record is at most 2^31 - 1 bytes
+    int rc = check_stream_ranges(n, src_len, 0x7FFFFFFFull, dst_off, dst_cap, d_src, d_dst, bytes, room);
+    if (rc) return rc;
     FrameReadScratch* s;
-    int rc = get_frame_read_scratch(&s);
+    rc = get_frame_read_scratch(&s);
     const WithLengthLayout L(n);
     if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
     if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
@@ -854,7 +757,7 @@ int64_t b200lz4f_compress_host_hc(const uint8_t* src, size_t n, uint8_t* dst, si
 int64_t b200lz4f_compress_host(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, int bsCode, int flags)
 { return b200lz4f_compress_host_hc(src, n, dst, cap, bsCode, flags, 0); }
 
-// the incremental writer (frame_writer_write_dev): host data only, no CUDA call in create or free
+// the incremental writer (writer_write_dev): host data only, no CUDA call in create or free
 void* b200lz4f_writer_create(size_t ns, int bsCode, int flags, int hc_level, const int64_t* known_size, int* err)
 {
     if (err) *err = 0;
@@ -865,27 +768,20 @@ void* b200lz4f_writer_create(size_t ns, int bsCode, int flags, int hc_level, con
         if (ns && !known_size) return fail("known_size is needed with flags bit 2");
         for (size_t k = 0; k < ns; k++) if (known_size[k] < 0) return fail("known_size must be >= 0");
     }
-    b200::FrameWriterHandle* h = new (std::nothrow) b200::FrameWriterHandle;
-    if (!h) return fail("out of host memory");
-    h->ns = ns; h->bsCode = bsCode; h->flags = flags; h->hc_level = hc_level;
-    try {
-        if (flags & 4) h->known.assign((const uint64_t*)known_size, (const uint64_t*)known_size + ns);
-        b200::FrameWriterState w{};                 // XXH32 with seed 0, nothing hashed yet (xxhash.c:445-455)
-        w.xxh.v[0] = 2654435761u + 2246822519u; w.xxh.v[1] = 2246822519u; w.xxh.v[2] = 0; w.xxh.v[3] = 0u - 2654435761u;
-        h->st.assign(ns, w);
-    } catch (...) { delete h; return fail("out of host memory"); }
-    return h;
+    void* h = b200::new_writer(b200::Container::Frame, ns, 1ull << (8 + 2 * bsCode), bsCode, flags, hc_level,
+                               (flags & 4) ? known_size : nullptr);
+    return h ? h : fail("out of host memory");
 }
 
 int b200lz4f_writer_write_dev(void* writer, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
                               const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
                               int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream)
 {
-    return b200::frame_writer_write_dev((b200::FrameWriterHandle*)writer, d_src, src_off, src_len, op, d_dst, dst_off, dst_cap,
-                                        status, src_consumed, produced, need, (cudaStream_t)stream);
+    return b200::writer_write_dev((b200::WriterHandle*)writer, d_src, src_off, src_len, op, d_dst, dst_off, dst_cap, status,
+                                  src_consumed, produced, need, (cudaStream_t)stream);
 }
 
-void b200lz4f_writer_free(void* writer) { delete (b200::FrameWriterHandle*)writer; }
+void b200lz4f_writer_free(void* writer) { delete (b200::WriterHandle*)writer; }
 
 // ---------------------------------------------------------------- "LZ4Block" container
 size_t b200lz4block_compress_bound(size_t n, int blockSize)
@@ -956,7 +852,7 @@ int b200lz4block_decompress_dev(const uint8_t* d_src, const uint64_t* src_off, c
                                          src_consumed, content_len, (cudaStream_t)stream);
 }
 
-// the incremental writer and reader (lz4block_writer_write_dev, lz4block_reader_read_dev): host data only, no CUDA call in
+// the incremental writer and reader (writer_write_dev, lz4block_reader_read_dev): host data only, no CUDA call in
 // create or free
 void* b200lz4block_writer_create(size_t ns, int blockSize, int hc_level, int* err)
 {
@@ -964,23 +860,20 @@ void* b200lz4block_writer_create(size_t ns, int blockSize, int hc_level, int* er
     auto fail = [&](const char* what) -> void* { const int rc = b200::fail_arg(what); if (err) *err = rc; return nullptr; };
     if (blockSize < 64 || blockSize > (1 << 25)) return fail("blockSize must be 64..32 MiB");
     if (ns > 0x7FFFFFFFull) return fail("too many streams in one writer");
-    b200::Lz4BlockWriterHandle* h = new (std::nothrow) b200::Lz4BlockWriterHandle;
-    if (!h) return fail("out of host memory");
-    h->ns = ns; h->bs = (uint64_t)blockSize; h->level = b200::lz4block_level(blockSize); h->hc_level = hc_level;
-    try { h->done.assign(ns, 0); }
-    catch (...) { delete h; return fail("out of host memory"); }
-    return h;
+    void* h = b200::new_writer(b200::Container::LZ4Block, ns, (uint64_t)blockSize, b200::lz4block_level(blockSize), 0, hc_level,
+                               nullptr);
+    return h ? h : fail("out of host memory");
 }
 
 int b200lz4block_writer_write_dev(void* writer, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len,
                                   const uint8_t* op, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
                                   int32_t* status, uint64_t* src_consumed, uint64_t* produced, uint64_t* need, void* stream)
 {
-    return b200::lz4block_writer_write_dev((b200::Lz4BlockWriterHandle*)writer, d_src, src_off, src_len, op, d_dst, dst_off,
-                                           dst_cap, status, src_consumed, produced, need, (cudaStream_t)stream);
+    return b200::writer_write_dev((b200::WriterHandle*)writer, d_src, src_off, src_len, op, d_dst, dst_off, dst_cap, status,
+                                  src_consumed, produced, need, (cudaStream_t)stream);
 }
 
-void b200lz4block_writer_free(void* writer) { delete (b200::Lz4BlockWriterHandle*)writer; }
+void b200lz4block_writer_free(void* writer) { delete (b200::WriterHandle*)writer; }
 
 void* b200lz4block_reader_create(size_t ns, int stopOnEmptyBlock, int* err)
 {

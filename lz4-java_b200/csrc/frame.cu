@@ -360,7 +360,6 @@ static int stream_payload_launches(const FrameStreamRead& r, uint8_t* slots, uin
                                    uint64_t nbsum, uint64_t nf, uint64_t nfsum, SideStream* side, cudaStream_t st,
                                    Xxh32Carry* carry = nullptr, const uint8_t* mode = nullptr)
 {
-    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     const uint64_t nb = nc + nr;
     if (nc) CK(cudaMemsetAsync(r.c_res, 0x80, nc * 4, st));                  // FRAME_RES_PENDING
     if (nf) CK(counted(launch_xxh32(r.src, r.h_off, r.h_len, 0, r.h_out, (size_t)nf, st)));
@@ -396,15 +395,11 @@ static int frame_streams_decompress_dev(const uint8_t* d_src, const uint64_t* sr
     if (ns == 0) return 0;
     if (!src_off || !src_len || !dst_off || !dst_cap || !result) return fail_arg("null pointer");
     if (ns > 0x7FFFFFFFull) return fail_arg("too many streams in one call");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < ns; k++) {
-        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
-        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    uint64_t bytes, room;
+    int rc = check_stream_ranges(ns, src_len, 1ull << 47, dst_off, dst_cap, d_src, d_dst, bytes, room);
+    if (rc) return rc;
     FrameReadScratch* s; SideStream* side;
-    int rc = get_frame_read_scratch(&s, &side);
+    rc = get_frame_read_scratch(&s, &side);
     const FrameStreamLayout L(ns);
     if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
     if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
@@ -443,7 +438,6 @@ static int frame_streams_decompress_dev(const uint8_t* d_src, const uint64_t* sr
     uint8_t* slots = s->d_slots;
     bind_stream_records(r, s->d_recs, R);
 
-    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     CK(counted(launch_frame_streams_walk(r, true, st)));
     rc = stream_payload_launches(r, slots, bytes, nc, nr, nbsum, nf, nfsum, side, st);
     if (rc) return rc;
@@ -492,15 +486,11 @@ static int frame_reader_read_dev(FrameReaderHandle* h, const uint8_t* d_src, con
     if (ns == 0) return 0;
     if (!src_off || !src_len || !eof || !dst_off || !dst_cap || !status || !src_consumed || !produced || !need)
         return fail_arg("null pointer");
-    uint64_t bytes = 0, room = 0;
-    for (size_t k = 0; k < ns; k++) {
-        if (src_len[k] > (1ull << 47) || dst_cap[k] > (1ull << 47)) return fail_arg("src_len / dst_cap");
-        if (dst_off[k] > ~0ull - dst_cap[k]) return fail_arg("a destination range overflows");
-        bytes += src_len[k]; room += dst_cap[k];
-    }
-    if ((bytes && !d_src) || (room && !d_dst)) return fail_arg("null pointer");
+    uint64_t bytes, room;
+    int rc = check_stream_ranges(ns, src_len, 1ull << 47, dst_off, dst_cap, d_src, d_dst, bytes, room);
+    if (rc) return rc;
     FrameReadScratch* s; SideStream* side;
-    int rc = get_frame_read_scratch(&s, &side);
+    rc = get_frame_read_scratch(&s, &side);
     const FrameReaderLayout L(ns);
     if (!rc) rc = reserve_device(s->d_seg, s->seg_cap, L.bytes);
     if (!rc) rc = reserve_pinned(s->h_seg, s->h_seg_cap, L.bytes);
@@ -550,7 +540,6 @@ static int frame_reader_read_dev(FrameReaderHandle* h, const uint8_t* d_src, con
     q.k_at = (uint64_t*)(B + k_at); q.fr_at = (uint64_t*)(B + fr_at); q.fr_end_at = (uint64_t*)(B + fr_end_at);
     q.fr_mode = (uint32_t*)(B + fr_mode); q.f_carry = (Xxh32Carry*)(B + f_carry); q.f_mode = B + f_mode;
 
-    auto counted = [](cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; };
     CK(counted(launch_frame_reader_walk(q, true, st)));
     rc = stream_payload_launches(r, slots, bytes, nc, nr, nbsum, nf, nfsum, side, st, q.f_carry, q.f_mode);
     if (rc) return rc;

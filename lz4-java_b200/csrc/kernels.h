@@ -100,7 +100,7 @@ cudaError_t launch_frame_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaS
 // every item: headers, block checksums, EndMarks, content checksums, f_off / f_end (frame_seal_kernel)
 cudaError_t launch_frame_seal(const FramePlan& p, cudaStream_t st);
 
-// The incremental frame writer (b200lz4f_writer_*: frame_writer_write_dev in containers.cu, kernels in frame_writer.cu).  One
+// The incremental frame writer (b200lz4f_writer_*: writer_write_dev in containers.cu, kernels in frame_writer.cu).  One
 // call is the frame writer's plan and chunk loop over the streams that write something: a "frame" of the plan is one such
 // stream's part of the call (its blocks, or one item without a block), with the header only on the stream's first call
 // (WRITER_HEAD) and the EndMark and content checksum only at its close (WRITER_TAIL).  Each stream's bytes go to its own
@@ -349,9 +349,9 @@ cudaError_t launch_lz4block_sizes(const FramePlan& p, uint32_t i0, uint32_t n, c
 cudaError_t launch_lz4block_emit(const FramePlan& p, uint32_t i0, uint32_t n, cudaStream_t st);
 // every item: block checksums (b_sum, masked to 28 bits), end blocks, f_off / f_end
 cudaError_t launch_lz4block_seal(const FramePlan& p, cudaStream_t st);
-// The incremental LZ4Block writer (b200lz4block_writer_*: lz4block_writer_write_dev in containers.cu): the incremental frame
-// writer's plan (FrameWriterPlan) with lz4block.cu's writer kernels.  No header is ever due; WRITER_TAIL puts the end block
-// on the plan frame's last item.
+// The incremental LZ4Block writer (b200lz4block_writer_*: writer_write_dev in containers.cu, as for frames): the incremental
+// frame writer's plan (FrameWriterPlan) with lz4block.cu's writer kernels.  No header is ever due; WRITER_TAIL puts the end
+// block on the plan frame's last item.  p.f_len is not read.
 cudaError_t launch_lz4block_writer_sizes(const FrameWriterPlan& w, uint32_t i0, uint32_t n, cudaStream_t st);
 cudaError_t launch_lz4block_writer_emit(const FrameWriterPlan& w, uint32_t i0, uint32_t n, cudaStream_t st);
 // every item: block checksums, end blocks, f_off / f_end as the stream's range written
@@ -500,12 +500,19 @@ static inline uint64_t compress_bound(uint64_t len) { return len + len / 255 + 1
 static inline uint64_t aligned_compress_bound(uint64_t len) { return (compress_bound(len) + 15) & ~uint64_t(15); }
 
 extern std::atomic<unsigned long long> g_launch_count;      // every kernel launch the library makes (any thread): b200lz4_launch_count()
+// one launch's result, the launch counted
+static inline cudaError_t counted(cudaError_t e) { g_launch_count.fetch_add(1, std::memory_order_relaxed); return e; }
 
 // ---- host layer shared by capi.cu, containers.cu and frame.cu
 extern const size_t CHUNK_SPAN;                            // bytes of source per chunk of a chunked call (B200LZ4_CHUNK_MB, default 256)
 static constexpr size_t CHUNK_BLOCKS = 1 << 16;            // blocks per chunk at most
 int fail_arg(const char* what);                            // set the thread's error message, return B200LZ4_E_ARG
 int fail_cuda(cudaError_t e, const char* where);           // ... B200LZ4_E_CUDA or _NODEVICE
+// The ranges of a device call over ns streams (or records): every src_len[k] at most src_max, every dst_cap[k] at most 2^47,
+// no dst_off[k] + dst_cap[k] past 2^64, and d_src / d_dst not NULL when the streams have bytes / room.  0 with the summed
+// lengths and capacities in bytes and room, or B200LZ4_E_ARG.
+int check_stream_ranges(size_t ns, const uint64_t* src_len, uint64_t src_max, const uint64_t* dst_off, const uint64_t* dst_cap,
+                        const void* d_src, const void* d_dst, uint64_t& bytes, uint64_t& room);
 // a failed CUDA call: the thread's error message names it, the caller returns fail_cuda's code
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return b200::fail_cuda(e_, #call); } while (0)
 int reserve_device(uint8_t*& p, size_t& cap, size_t need, int slack_shift = 2);   // grow-or-keep device buffer

@@ -146,14 +146,7 @@ def decompress_frame_streams_dev(src, src_off, src_len, out, dst_off, dst_cap, r
     reader stopped (0 on an error), and what it decodes to when room is not the limit.  Raises only on a backend error."""
     import torch
     off, ln = _dev_streams(src, src_off, src_len, "stream")
-    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
-        raise ValueError("out must be a contiguous uint8 tensor on src's device")
-    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
-    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
-    if len(doff) != len(ln) or len(dcap) != len(ln):
-        raise ValueError("dst_off and dst_cap must have one entry per stream")
-    if len(ln) and int((doff + dcap).max()) > out.numel():
-        raise ValueError("a destination range reaches past the end of out")
+    doff, dcap = _dev_ranges(src, out, dst_off, dst_cap, len(ln), "stream")
     result = np.zeros(len(ln), dtype=np.int64)
     consumed, content = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
     N.check(N.lib().b200lz4f_decompress_streams_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
@@ -337,6 +330,20 @@ def _dev_streams(src, src_off, src_len, what):
     return off, ln
 
 
+def _dev_ranges(src, out, dst_off, dst_cap, n, what):
+    """the host destination offset / capacity arrays of a device call over n streams (or records) of src, checked against out"""
+    import torch
+    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous uint8 tensor on src's device")
+    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
+    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
+    if len(doff) != n or len(dcap) != n:
+        raise ValueError(f"dst_off and dst_cap must have one entry per {what}")
+    if n and int((doff + dcap).max()) > out.numel():
+        raise ValueError("a destination range reaches past the end of out")
+    return doff, dcap
+
+
 def compress_lz4block_dev(src, src_off, src_len, block_size: int = 1 << 16, hc_level: int = 0, out=None):
     """independent LZ4Block streams of bytes already in device memory, written on the device (b200lz4block_compress_dev):
     stream s is src[src_off[s] : src_off[s] + src_len[s]], byte for byte what compress_lz4block writes for the same bytes at
@@ -373,14 +380,7 @@ def decompress_lz4block_dev(src, src_off, src_len, out, dst_off, dst_cap, stop_o
     read (0 on an error), and what it decodes to when room is not the limit.  Raises only on a backend error."""
     import torch
     off, ln = _dev_streams(src, src_off, src_len, "stream")
-    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
-        raise ValueError("out must be a contiguous uint8 tensor on src's device")
-    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
-    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
-    if len(doff) != len(ln) or len(dcap) != len(ln):
-        raise ValueError("dst_off and dst_cap must have one entry per stream")
-    if len(ln) and int((doff + dcap).max()) > out.numel():
-        raise ValueError("a destination range reaches past the end of out")
+    doff, dcap = _dev_ranges(src, out, dst_off, dst_cap, len(ln), "stream")
     result = np.zeros(len(ln), dtype=np.int64)
     consumed, content = np.zeros(len(ln), dtype=np.uint64), np.zeros(len(ln), dtype=np.uint64)
     N.check(N.lib().b200lz4block_decompress_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
@@ -526,14 +526,7 @@ def decompress_with_length_dev(src, src_off, src_len, out, dst_off, dst_cap, saf
     (-1 when the record is shorter than 4 bytes).  Raises only on a backend error."""
     import torch
     off, ln = _dev_streams(src, src_off, src_len, "record")
-    if not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != src.device or not out.is_contiguous():
-        raise ValueError("out must be a contiguous uint8 tensor on src's device")
-    doff = np.ascontiguousarray(np.asarray(dst_off, dtype=np.uint64).reshape(-1))
-    dcap = np.ascontiguousarray(np.asarray(dst_cap, dtype=np.uint64).reshape(-1))
-    if len(doff) != len(ln) or len(dcap) != len(ln):
-        raise ValueError("dst_off and dst_cap must have one entry per record")
-    if len(ln) and int((doff + dcap).max()) > out.numel():
-        raise ValueError("a destination range reaches past the end of out")
+    doff, dcap = _dev_ranges(src, out, dst_off, dst_cap, len(ln), "record")
     result, orig_len = np.zeros(len(ln), dtype=np.int64), np.zeros(len(ln), dtype=np.int64)
     N.check(N.lib().b200lz4_decompress_with_length_dev(src.data_ptr(), off.ctypes.data, ln.ctypes.data, len(ln), out.data_ptr(),
                                                        doff.ctypes.data, dcap.ctypes.data, int(bool(safe)), result.ctypes.data,

@@ -336,7 +336,8 @@ def test_device_round_trip_at_scale(b200, port):
 
 def test_errors_launch_nothing_and_write_nothing(b200, port):
     """writer: dst_capacity one short of the bounds (-9), blockSize 63 and 32 MiB + 1 (B200LZ4_E_ARG), no streams (0);
-    reader: a NULL result array, NULL offsets (B200LZ4_E_ARG), no streams (0): no launch, no byte written"""
+    reader: a NULL result array, NULL offsets, a destination range that overflows (B200LZ4_E_ARG; the stream is only its end
+    block, so nothing would be written), no streams (0): no launch, no byte written"""
     L, M = b200._native.lib(), _DevMem()
     datas = [port.datagen(100000, 0.5, 0.0, 6).tobytes(), b"xyz"]
     src, offs, lens = _lay_out(datas)
@@ -352,6 +353,8 @@ def test_errors_launch_nothing_and_write_nothing(b200, port):
     assert _read(L, M, d_src, offs, lens, d_dst, doff, dcap, True, result=False)[0] == E_ARG
     assert L.b200lz4block_decompress_dev(M.ptr(d_src), None, lens.ctypes.data, 2, M.ptr(d_dst), doff.ctypes.data, dcap.ctypes.data,
                                          1, np.zeros(2, dtype=np.int64).ctypes.data, None, None, None) == E_ARG
+    d_end = M.up(np.frombuffer(_header(0x10, 0, 0, 0, 0), dtype=np.uint8))
+    assert _read(L, M, d_end, _u64([0]), _u64([21]), d_dst, _u64([2**64 - 2]), _u64([16]), True)[0] == E_ARG
     assert _read(L, M, d_src, offs[:0], lens[:0], d_dst, doff[:0], dcap[:0], True)[0] == 0
     assert L.b200lz4_launch_count() == before
     assert (M.down(d_dst) == END_GUARD).all()

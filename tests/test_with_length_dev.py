@@ -307,8 +307,9 @@ def test_round_trip_with_the_writer(b200, port):
 
 def test_errors_launch_nothing_and_write_nothing(b200, port):
     """writer: dst_capacity one short of the bounds (-9), a record of 0x7E000001 bytes, NULL source or destination
-    (B200LZ4_E_ARG), no records (0); reader: a NULL result array, NULL offsets, a record of 2^31 bytes (B200LZ4_E_ARG), no
-    records (0): no launch, no byte written"""
+    (B200LZ4_E_ARG), no records (0); reader: a NULL result array, NULL offsets, a record of 2^31 bytes, a destination range
+    that overflows (B200LZ4_E_ARG; the record declares length 0, so nothing would be written), no records (0): no launch, no
+    byte written"""
     L, M = b200._native.lib(), _DevMem()
     datas = [port.datagen(100000, 0.5, 0.0, 6).tobytes(), b"xyz"]
     src, offs, lens = _lay_out(datas)
@@ -330,6 +331,8 @@ def test_errors_launch_nothing_and_write_nothing(b200, port):
     assert L.b200lz4_decompress_with_length_dev(M.ptr(d_src), None, lens.ctypes.data, 2, M.ptr(d_dst), doff.ctypes.data,
                                                 dcap.ctypes.data, 1, res.ctypes.data, None, None) == E_ARG
     assert _read(L, M, d_src, offs, _u64([1 << 31, 3]), d_dst, doff, dcap, True)[0] == E_ARG
+    d_empty = M.up(np.zeros(5, dtype=np.uint8))                   # length 0, then the empty block's one token
+    assert _read(L, M, d_empty, _u64([0]), _u64([5]), d_dst, _u64([2**64 - 2]), _u64([16]), False)[0] == E_ARG
     assert _read(L, M, d_src, offs[:0], lens[:0], d_dst, doff[:0], dcap[:0], True)[0] == 0
     assert L.b200lz4_launch_count() == before
     assert (M.down(d_dst) == END_GUARD).all()
